@@ -5,8 +5,8 @@ GPU mode against GPU mode:
 
   * config 2: the entire 4 194 304-candidate cube, status bytes and winners;
   * configs 3, 4 (2 000-server slice) and 5 (A = 16 slice), generated exactly as bench.py generates them and
-    swept by the kernels bench.py's default path uses for shards of that size (k_grid_rows + the deferred
-    exact-chain kernels): >= 1e6 random candidates, EVERY candidate the sweep handed to the exact-chain
+    swept by bench.py's default path (k_scan_prep -> k_scan_cert || k_scan_lean + the deferred exact-chain
+    kernels): >= 1e6 random candidates, EVERY candidate the sweep handed to the exact-chain
     kernels, and every server's winner (its own record, plus an exhaustive proof that no candidate with a
     smaller key is feasible according to the oracle);
   * 1e7 random QueueAnalyzer.Analyze requests in certified mode, including the edges of the certificate's
@@ -48,7 +48,7 @@ def _decode(idx, A, R, B):
     return (pair // A).astype(np.int32), (pair % A).astype(np.int32), r, b
 
 
-def _check_sweep_against_oracle(wva, oracle, ctx, img, first, count, R, B, n_random, seed, expect_rows_kernel=True, also_fused=False):
+def _check_sweep_against_oracle(wva, oracle, ctx, img, first, count, R, B, n_random, seed, also_fused=False):
     """Sweep servers [first, first+count) of `img` on the GPU (cube + status + winners) and check against the oracle:
     random candidates, all deferred candidates, and the winners exhaustively.  Returns counters for the report.
     also_fused: sweep a second time the way a repeated reconcile does when the deferred list is long (no stop at the host
@@ -74,8 +74,6 @@ def _check_sweep_against_oracle(wva, oracle, ctx, img, first, count, R, B, n_ran
     assert n_def == len(deferred) == lists["deferred"]
     ncand = count * A * R * B
     assert len(cube) == ncand
-    if expect_rows_kernel:
-        assert count * A * R >= 32768, "shard too small: bench.py's default path would not use k_grid_rows here"
     # (1) random candidates + (2) every deferred candidate
     rng = np.random.default_rng(seed)
     idx = np.unique(np.concatenate([rng.integers(0, ncand, n_random).astype(np.uint64), deferred]))
@@ -120,7 +118,7 @@ def _check_sweep_against_oracle(wva, oracle, ctx, img, first, count, R, B, n_ran
 
 def test_config3_sweep_vs_oracle(wva, oracle, ctx):
     """BASELINE config 3 (bench.py's default workload): 1 000 servers x 8 accelerators x 64 x 512, swept in
-    250-server shards (so that the host copy of the cube stays at 2.2 GB) by k_grid_rows + deferred kernels."""
+    250-server shards (so that the host copy of the cube stays at 2.2 GB) by the default sweep kernels + deferred kernels."""
     img, c = wva.synth.baseline_config(3)
     tot = dict(checked=0, deferred=0, winners=0, proof_candidates=0)
     for first in range(0, img.S, 250):
