@@ -258,6 +258,32 @@ func (c *Context) AnalyzeGrid(s, rMax, bMax int) ([]GridBest, error) {
 	return best, c.err(rc, "wva_analyze_grid")
 }
 
+// GridBlocking returns the blocking probability p_block (float32 of the model's p[K], K = 11 b) of every candidate of
+// the last successful sweep, indexed like the metric cube over the shard; NaN where Analyze does not accept the
+// candidate.  The slice is sized by the library (wva_grid_blocking_size).  The plane also stays in HBM.
+func (c *Context) GridBlocking() ([]float32, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var n C.size_t
+	if err := c.err(C.wva_grid_blocking_size(c.ctx, &n), "wva_grid_blocking_size"); err != nil {
+		return nil, err
+	}
+	out := make([]float32, int(n))
+	return out, c.err(C.wva_grid_blocking(c.ctx, f32p(out)), "wva_grid_blocking")
+}
+
+// GridBestBlocking returns p_block of each server's sweep winner (s servers of the shard), NaN where no candidate is
+// feasible.  Needs neither the metric cube nor the plane of GridBlocking.
+func (c *Context) GridBestBlocking(s int) ([]float32, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	out := make([]float32, s)
+	if s == 0 {
+		return out, nil
+	}
+	return out, c.err(C.wva_grid_best_blocking(c.ctx, f32p(out)), "wva_grid_best_blocking")
+}
+
 // QueueConfig is wva_queue_config; Metrics is wva_metrics (analyzer.AnalysisMetrics).
 type QueueConfig struct {
 	MaxBatchSize, MaxQueueSize int32
@@ -372,6 +398,17 @@ func (g *Group) Analyze(rMax, bMax int) error {
 	g.mu.Lock()
 	defer g.mu.Unlock()
 	return g.err(C.wva_group_analyze(g.g, C.int32_t(rMax), C.int32_t(bMax), 0), "wva_group_analyze")
+}
+
+// GridBestBlocking: p_block of every server's sweep winner (s servers), assembled from the devices' shards.
+func (g *Group) GridBestBlocking(s int) ([]float32, error) {
+	g.mu.Lock()
+	defer g.mu.Unlock()
+	out := make([]float32, s)
+	if s == 0 {
+		return out, nil
+	}
+	return out, g.err(C.wva_group_grid_best_blocking(g.g, f32p(out)), "wva_group_grid_best_blocking")
 }
 
 // AllocateByType: global per-type totals (NCCL all-gather of the partials inside the library).

@@ -266,6 +266,31 @@ int wva_grid_fetch(wva_ctx* ctx, wva_grid_best* best);
  * sweep.  Reads must be ordered after that sweep (e.g. a device synchronisation). */
 int wva_grid_cube_device(wva_ctx* ctx, void** cube, void** status, size_t* n);
 
+/* Blocking probability (the share of requests turned away because the 10 b queue is full) of every candidate of the
+ * last sweep slice (same shard, r_max, b_max): p_block = float32(p[K]) of the reference's
+ * Analyze(totalRate / float32(r)) on NewQueueAnalyzer({b, 10 b}), K = 11 b, bit for bit, where the candidate's status is
+ * WVA_CAND_OK (feasible or not); the quiet NaN 0x7fc00000 for every other candidate.  Indexed like the cube:
+ * ((s*A+a)*r_max+(r-1))*b_max+(b-1) over the shard.  Works whether or not the sweep kept its cube.  The plane stays in
+ * HBM; p_block is a HOST array [servers of the shard x A x r_max x b_max] or NULL.  WVA_ESTATE when no sweep has run
+ * since the last upload, update or shard change. */
+int wva_grid_blocking(wva_ctx* ctx, float* p_block);
+/* Candidates of that plane (the extent of wva_grid_blocking's host array): servers of the shard x A x r_max x b_max of
+ * the last SUCCESSFUL sweep (a sweep call that fails leaves the previous one in place).  WVA_ESTATE like
+ * wva_grid_blocking. */
+int wva_grid_blocking_size(const wva_ctx* ctx, size_t* n);
+/* Device address of that plane (float[*n]); valid until the next sweep or wva_grid_blocking call, WVA_ESTATE when
+ * wva_grid_blocking has not run since the last sweep. */
+int wva_grid_blocking_device(wva_ctx* ctx, void** p_block, size_t* n);
+/* How the last plane was produced: out = {certified zero, certified closed form, exact chain} candidate counts. */
+int wva_grid_blocking_counts(const wva_ctx* ctx, int64_t out[3]);
+/* Candidate ids (cube indices relative to the shard) the last wva_grid_blocking ran as exact chains, the scan's list
+ * followed by the materialised-path list (an id may appear in both); at most cap are copied, *n = how many there were.
+ * A later wva_grid_best_blocking empties the second list.  Test/diagnostic aid. */
+int wva_grid_blocking_exact_fetch(wva_ctx* ctx, uint64_t* ids, int32_t cap, int32_t* n);
+/* p_block of each server's sweep winner (wva_grid_fetch), NaN where acc == -1; p_block is a HOST array [servers of the
+ * shard].  Needs neither the cube nor the plane (works for sweeps that keep winners only). */
+int wva_grid_best_blocking(wva_ctx* ctx, float* p_block);
+
 /* Both halves of Analyze in one call: wva_analyze_pairs and wva_analyze_grid_device are independent
  * and are run concurrently (the sweep on its own stream).  Results stay in HBM:
  * wva_pairs_fetch / wva_grid_fetch copy them out, wva_solve consumes the pair records in place. */
@@ -406,6 +431,7 @@ int wva_group_upload(wva_group* g, const wva_system_soa* host);      /* replicat
 int wva_group_analyze(wva_group* g, int32_t r_max, int32_t b_max, int32_t want_cube);   /* r_max = 0: pairs only */
 int wva_group_pairs_fetch(wva_group* g, wva_alloc_soa* out, uint8_t* feasible);
 int wva_group_grid_fetch(wva_group* g, wva_grid_best* best /* [S] */);
+int wva_group_grid_best_blocking(wva_group* g, float* p_block /* [S] */);   /* wva_grid_best_blocking, assembled */
 int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen);
 int wva_group_allocate_by_type(wva_group* g, int64_t* count, float* cost);
 

@@ -11,6 +11,10 @@ ABI_VERSION = 1
 
 OK, EINVAL, ECUDA, ESTATE, ENOSOLUTION, ENONFINITE, ECAPACITY = 0, -1, -2, -3, -4, -5, -6
 
+# wva_grid_blocking: p_block of a candidate Analyze does not accept is this quiet NaN; wva_grid_blocking_counts order
+BLOCK_NAN_BITS = 0x7fc00000
+BLOCK_COUNTS = ("zero", "closed_form", "exact")
+
 POLICY_NONE, POLICY_PRIORITY_EXHAUSTIVE, POLICY_PRIORITY_ROUND_ROBIN, POLICY_ROUND_ROBIN = 0, 1, 2, 3
 POLICY_BY_NAME = {  # SaturatedAllocationPolicyEnum, reference pkg/config/config.go:28-41
     "None": POLICY_NONE,

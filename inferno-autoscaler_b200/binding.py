@@ -29,6 +29,8 @@ EXPORTS = [
     "wva_comm_unique_id", "wva_comm_init", "wva_comm_destroy", "wva_comm_info", "wva_comm_shard",
     "wva_group_create", "wva_group_destroy", "wva_group_size", "wva_group_ctx", "wva_group_last_error", "wva_group_upload",
     "wva_group_analyze", "wva_group_pairs_fetch", "wva_group_grid_fetch", "wva_group_solve", "wva_group_allocate_by_type",
+    "wva_grid_blocking", "wva_grid_blocking_size", "wva_grid_blocking_device", "wva_grid_best_blocking", "wva_grid_blocking_counts", "wva_grid_blocking_exact_fetch",
+    "wva_group_grid_best_blocking",
 ]
 
 
@@ -122,6 +124,13 @@ def lib():
         L.wva_group_grid_fetch.argtypes = [vp, vp]
         L.wva_group_solve.argtypes = [vp, C.POINTER(abi.OptimizerSpec), abi.i32p, C.POINTER(abi.AllocSoa)]
         L.wva_group_allocate_by_type.argtypes = [vp, abi.i64p, abi.f32p]
+        L.wva_grid_blocking.argtypes = [vp, abi.f32p]
+        L.wva_grid_blocking_size.argtypes = [vp, C.POINTER(C.c_size_t)]
+        L.wva_grid_blocking_device.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t)]
+        L.wva_grid_best_blocking.argtypes = [vp, abi.f32p]
+        L.wva_grid_blocking_counts.argtypes = [vp, abi.i64p]
+        L.wva_grid_blocking_exact_fetch.argtypes = [vp, C.POINTER(u64), i32, C.POINTER(i32)]
+        L.wva_group_grid_best_blocking.argtypes = [vp, abi.f32p]
         if L.wva_abi_version() != abi.ABI_VERSION:
             raise ImportError("libwva_b200.so ABI version mismatch")
         _lib = L
@@ -356,6 +365,43 @@ class Context:
         self._ck(lib().wva_grid_cube_device(self._h, C.byref(cube), C.byref(status), C.byref(n)))
         return cube.value, status.value, n.value
 
+    def grid_blocking(self, download=True):
+        """Blocking probability p_block of every candidate of the last sweep (float32, cube order over the shard; the quiet
+        NaN where Analyze does not accept the candidate).  download=False leaves the plane on the device only."""
+        if not download:
+            self._ck(lib().wva_grid_blocking(self._h, None))
+            return None
+        n = C.c_size_t()
+        self._ck(lib().wva_grid_blocking_size(self._h, C.byref(n)))       # the library's extent, not the caller's
+        out = np.empty(n.value, dtype=np.float32)
+        self._ck(lib().wva_grid_blocking(self._h, abi.ptr(out, C.c_float)))
+        return out
+
+    def grid_blocking_device(self):
+        """(address, candidates) of the blocking-probability plane on the device"""
+        p, n = C.c_void_p(), C.c_size_t()
+        self._ck(lib().wva_grid_blocking_device(self._h, C.byref(p), C.byref(n)))
+        return p.value, n.value
+
+    def grid_blocking_counts(self):
+        """how the last plane was produced: candidates decided by the certified zero, the certified closed form, an exact chain"""
+        out = np.zeros(3, dtype=np.int64)
+        self._ck(lib().wva_grid_blocking_counts(self._h, abi.ptr(out, C.c_int64)))
+        return dict(zero=int(out[0]), closed_form=int(out[1]), exact=int(out[2]))
+
+    def grid_blocking_exact(self, cap=1 << 24):
+        """cube indices (relative to the shard) the last grid_blocking ran as exact chains (sorted, unique)"""
+        n = C.c_int32(0)
+        ids = np.zeros(cap, dtype=np.uint64)
+        self._ck(lib().wva_grid_blocking_exact_fetch(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint64)), cap, C.byref(n)))
+        return np.unique(ids[:min(n.value, cap)]), n.value
+
+    def grid_best_blocking(self):
+        """p_block of each server's sweep winner (NaN where no candidate is feasible), [servers of the shard]"""
+        out = np.empty(self.count, dtype=np.float32)
+        self._ck(lib().wva_grid_best_blocking(self._h, abi.ptr(out, C.c_float)))
+        return out
+
     def grid_set_tail_cap(self, cap):
         self._ck(lib().wva_grid_set_tail_cap(self._h, int(cap)))
 
@@ -520,6 +566,12 @@ class Group:
         best = np.zeros(self.image.S, dtype=abi.GRID_BEST_DTYPE)
         self._ck(lib().wva_group_grid_fetch(self._h, best.ctypes.data))
         return best
+
+    def grid_best_blocking(self):
+        """p_block of every server's sweep winner, assembled from the devices' shards [S]"""
+        out = np.empty(self.image.S, dtype=np.float32)
+        self._ck(lib().wva_group_grid_best_blocking(self._h, abi.ptr(out, C.c_float)))
+        return out
 
     def solve(self, unlimited=True, delayed_best_effort=False, policy=abi.POLICY_NONE, download=True):
         spec = abi.OptimizerSpec(1 if unlimited else 0, 1 if delayed_best_effort else 0, int(policy))

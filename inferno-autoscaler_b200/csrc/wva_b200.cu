@@ -3,7 +3,9 @@
 // One ctx = one CUDA device + one stream.  All entry points launch kernels; there is no host
 // implementation of any arithmetic in this file (and no fallback when CUDA is unavailable).
 #include "wva_kernels.cuh"
+#include "wva_block.cuh"
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -213,11 +215,19 @@ struct wva_ctx {
     mutable bool pendS = false, pendT = false;
     int grid_r = 0, grid_b = 0; bool grid_valid = false;
     bool grid_has_cube = false;          // the last sweep wrote the metric cube and the status bytes
+    uint64_t grid_epoch = 0;             // completed sweeps: tells a blocking plane whose sweep it belongs to
     uint64_t grid_counters[3] = {0, 0, 0};
 
     // multi-rank exchange (wva_comm_init / wva_group_create)
     nccl_comm_t comm = nullptr; int comm_rank = 0, comm_size = 1; bool comm_owned = false;
     DevBuf commTotals, commChunk, commGather;
+
+    // blocking probability of the sweep's candidates (wva_grid_blocking*)
+    DevBuf blkPlane, blkExact, blkLit, blkCount, blkCounts, blkScratch, blkIo;
+    size_t blk_exact_cap = 0, blk_lit_cap = 0;
+    size_t blk_exact_n = 0, blk_lit_n = 0;  // list lengths of the last plane (the scan's exact list, the whole literal list)
+    bool blk_valid = false; uint64_t blk_epoch = 0;
+    int64_t blk_counts[3] = {0, 0, 0};
 
     // misc io buffers for the low-level API
     DevBuf ioA, ioB, ioC, ioD, ioE, ioF, ioG;
@@ -391,7 +401,8 @@ void wva_ctx_destroy(wva_ctx* ctx) {
                       &ctx->greedyBuf, &ctx->keys, &ctx->bestDev, &ctx->cube, &ctx->status, &ctx->counters,
                       &ctx->gridSlow, &ctx->gridSlowCount, &ctx->faultList, &ctx->faultCount, &ctx->heavyList, &ctx->heavyCost,
                       &ctx->heavyOrder, &ctx->heavyHist, &ctx->pairTab, &ctx->blockSlot, &ctx->listSlot, &ctx->gscratch, &ctx->rowInfo, &ctx->rateTab, &ctx->ioA, &ctx->ioB,
-                      &ctx->ioC, &ctx->ioD, &ctx->ioE, &ctx->ioF, &ctx->ioG, &ctx->commTotals, &ctx->commChunk, &ctx->commGather};
+                      &ctx->ioC, &ctx->ioD, &ctx->ioE, &ctx->ioF, &ctx->ioG, &ctx->commTotals, &ctx->commChunk, &ctx->commGather,
+                      &ctx->blkPlane, &ctx->blkExact, &ctx->blkLit, &ctx->blkCount, &ctx->blkCounts, &ctx->blkScratch, &ctx->blkIo};
     for (DevBuf* b : bufs) b->release();
     ctx->staging.release();
     cudaEventDestroy(ctx->ev0);
@@ -1091,6 +1102,7 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
     }
     ctx->grid_r = r_max; ctx->grid_b = b_max; ctx->grid_valid = true;
     ctx->grid_has_cube = want_cube && want_status;
+    ctx->grid_epoch++;
     return WVA_OK;
 }
 
@@ -1221,6 +1233,176 @@ int wva_grid_counters(const wva_ctx* ctx, uint64_t* steps_executed, uint64_t* st
     if (steps_executed) *steps_executed = ctx->grid_counters[0];
     if (steps_algorithmic) *steps_algorithmic = ctx->grid_counters[1];
     if (candidates_ok) *candidates_ok = ctx->grid_counters[2];
+    return WVA_OK;
+}
+
+// ---- blocking probability of the sweep's candidates (wva_block.cuh) --------------------------------------------------
+// Everything runs on the main stream, after the sweep (which joins it), on buffers of its own: the sweep's cube, status
+// bytes, winners and lists are only read.
+static BlockParams block_params(wva_ctx* ctx) {
+    BlockParams bp;
+    bp.r_max = ctx->grid_r; bp.b_max = ctx->grid_b; bp.s0 = ctx->s0; bp.ns = ctx->ns;
+    bp.plane = ctx->blkPlane.as<float>();
+    bp.exact_list = ctx->blkExact.as<unsigned long long>();
+    bp.exact_cap = ctx->blkExact.cap / 8;
+    bp.lit_list = ctx->blkLit.as<unsigned long long>();
+    bp.lit_cap = ctx->blkLit.cap / 8;
+    bp.list_count = ctx->blkCount.as<unsigned long long>();
+    bp.counts = ctx->blkCounts.as<unsigned long long>();
+    return bp;
+}
+
+// Exact chains of list[0, n), then the candidates whose chain met a rescale predicate (and those the scan listed) on
+// the materialised path, in pieces whose p[] scratch fits in half of the free device memory.  The literal list must
+// have room for n more entries than it holds.
+static int block_finish(wva_ctx* ctx, const BlockParams& bp, const unsigned long long* list, size_t n, float* out, int byServer) {
+    if (n > 0x7fffffffULL) return fail(ctx, WVA_EINVAL, "blocking: more than 2^31 - 1 exact chains");
+    if (n > 0) {
+        k_block_exact<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(ctx->dsys, bp, list, (int)n, out, byServer);
+        LAUNCH_CHECK();
+    }
+    unsigned long long lit = 0;
+    CK(cudaMemcpyAsync(&lit, bp.list_count + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (lit > bp.lit_cap) return fail(ctx, WVA_ECUDA, "blocking: literal list overflow");
+    if (lit == 0) return WVA_OK;
+    const long long stride = 11LL * bp.b_max + 1;
+    const size_t per = (size_t)stride * 8;
+    size_t freeB = 0, totB = 0;
+    CK(cudaMemGetInfo(&freeB, &totB));
+    size_t maxItems = std::max<size_t>(ctx->blkScratch.cap / per, (freeB / 2) / per);
+    if (maxItems == 0) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
+    if (maxItems > (size_t)lit) maxItems = (size_t)lit;
+    CK(ctx->blkScratch.ensure(maxItems * per));
+    for (size_t done = 0; done < (size_t)lit; done += maxItems) {
+        const int m = (int)std::min<size_t>((size_t)lit - done, maxItems);
+        k_block_literal<<<(m + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, bp, bp.lit_list + done, m, ctx->blkScratch.as<double>(),
+                                                                  stride, out, byServer);
+        LAUNCH_CHECK();
+    }
+    return WVA_OK;
+}
+
+int wva_grid_blocking_size(const wva_ctx* ctx, size_t* n) {
+    if (!ctx || !n) return WVA_EINVAL;
+    if (!ctx->grid_valid) return fail(const_cast<wva_ctx*>(ctx), WVA_ESTATE, "no grid sweep has run since the last upload or update");
+    *n = (size_t)ctx->ns * ctx->A * (size_t)ctx->grid_r * (size_t)ctx->grid_b;
+    return WVA_OK;
+}
+
+int wva_grid_blocking(wva_ctx* ctx, float* p_block) {
+    if (!ctx) return WVA_EINVAL;
+    if (!ctx->grid_valid) return fail(ctx, WVA_ESTATE, "no grid sweep has run since the last upload or update");
+    CK(cudaSetDevice(ctx->device));
+    ctx->blk_valid = false;
+    const size_t nRows = (size_t)ctx->ns * ctx->A * (size_t)ctx->grid_r;
+    const size_t nCand = nRows * (size_t)ctx->grid_b;
+    CK(ctx->blkPlane.ensure(nCand ? nCand * 4 : 4));
+    CK(ctx->blkCount.ensure(2 * 8));
+    CK(ctx->blkCounts.ensure(3 * 8));
+    if (ctx->blk_exact_cap == 0) ctx->blk_exact_cap = std::max<size_t>(1, std::min<size_t>(nCand, (size_t)1 << 20));
+    if (ctx->blk_lit_cap == 0) ctx->blk_lit_cap = (size_t)1 << 16;
+    unsigned long long counts[2] = {0, 0};
+    BlockParams bp;
+    for (;;) {
+        CK(ctx->blkExact.ensure((size_t)ctx->blk_exact_cap * 8));
+        CK(ctx->blkLit.ensure((size_t)ctx->blk_lit_cap * 8));
+        bp = block_params(ctx);
+        CK(cudaMemsetAsync(ctx->blkCount.p, 0, 2 * 8, ctx->stream));
+        CK(cudaMemsetAsync(ctx->blkCounts.p, 0, 3 * 8, ctx->stream));
+        if (nRows > 0) {
+            k_block_scan<<<(unsigned)((nRows + 127) / 128), 128, 0, ctx->stream>>>(ctx->dsys, bp);
+            LAUNCH_CHECK();
+        }
+        CK(cudaMemcpyAsync(counts, ctx->blkCount.p, 2 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        // the literal list also takes every exact chain that meets a rescale predicate
+        const unsigned long long needLit = counts[0] + counts[1];
+        if (counts[0] <= bp.exact_cap && needLit <= bp.lit_cap) break;
+        if (needLit > 0x7fffffffULL) return fail(ctx, WVA_EINVAL, "blocking: more than 2^31 - 1 exact chains");
+        ctx->blk_exact_cap = std::max<size_t>(ctx->blk_exact_cap, counts[0]);     // rare: lists outgrew their buffers, scan again
+        ctx->blk_lit_cap = std::max<size_t>(ctx->blk_lit_cap, needLit);
+    }
+    int rc = block_finish(ctx, bp, bp.exact_list, counts[0], bp.plane, 0);
+    if (rc != WVA_OK) return rc;
+    unsigned long long lit = 0;
+    CK(cudaMemcpyAsync(&lit, bp.list_count + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    uint64_t c[3] = {0, 0, 0};
+    CK(cudaMemcpyAsync(c, ctx->blkCounts.p, 3 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (p_block && nCand) CK(cudaMemcpyAsync(p_block, ctx->blkPlane.p, nCand * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < 3; ++k) ctx->blk_counts[k] = (int64_t)c[k];
+    ctx->blk_exact_n = counts[0]; ctx->blk_lit_n = lit;
+    ctx->blk_valid = true; ctx->blk_epoch = ctx->grid_epoch;
+    return WVA_OK;
+}
+
+int wva_grid_blocking_exact_fetch(wva_ctx* ctx, uint64_t* ids, int32_t cap, int32_t* n) {
+    if (!ctx || !n || cap < 0 || (cap > 0 && !ids)) return WVA_EINVAL;
+    if (!ctx->grid_valid || !ctx->blk_valid || ctx->blk_epoch != ctx->grid_epoch)
+        return fail(ctx, WVA_ESTATE, "wva_grid_blocking has not run since the last grid sweep");
+    const size_t total = ctx->blk_exact_n + ctx->blk_lit_n;
+    *n = (int32_t)std::min<size_t>(total, 0x7fffffff);
+    const size_t k1 = std::min<size_t>(ctx->blk_exact_n, (size_t)cap), k2 = std::min<size_t>(ctx->blk_lit_n, (size_t)cap - k1);
+    CK(cudaSetDevice(ctx->device));
+    if (k1 > 0) CK(cudaMemcpyAsync(ids, ctx->blkExact.p, (size_t)k1 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (k2 > 0) CK(cudaMemcpyAsync(ids + k1, ctx->blkLit.p, (size_t)k2 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return WVA_OK;
+}
+
+int wva_grid_blocking_device(wva_ctx* ctx, void** p_block, size_t* n) {
+    if (!ctx || !p_block || !n) return WVA_EINVAL;
+    if (!ctx->grid_valid || !ctx->blk_valid || ctx->blk_epoch != ctx->grid_epoch)
+        return fail(ctx, WVA_ESTATE, "wva_grid_blocking has not run since the last grid sweep");
+    *p_block = ctx->blkPlane.p;
+    *n = (size_t)ctx->ns * ctx->A * (size_t)ctx->grid_r * (size_t)ctx->grid_b;
+    return WVA_OK;
+}
+
+int wva_grid_blocking_counts(const wva_ctx* ctx, int64_t out[3]) {
+    if (!ctx || !out) return WVA_EINVAL;
+    if (!ctx->grid_valid || !ctx->blk_valid || ctx->blk_epoch != ctx->grid_epoch)
+        return fail(const_cast<wva_ctx*>(ctx), WVA_ESTATE, "wva_grid_blocking has not run since the last grid sweep");
+    for (int k = 0; k < 3; ++k) out[k] = ctx->blk_counts[k];
+    return WVA_OK;
+}
+
+int wva_grid_best_blocking(wva_ctx* ctx, float* p_block) {
+    if (!ctx || !p_block) return WVA_EINVAL;
+    if (!ctx->grid_valid) return fail(ctx, WVA_ESTATE, "no grid sweep has run since the last upload or update");
+    const int ns = ctx->ns;
+    if (ns == 0) return WVA_OK;
+    CK(cudaSetDevice(ctx->device));
+    std::vector<wva_grid_best> best((size_t)ns);
+    CK(cudaMemcpyAsync(best.data(), ctx->bestDev.p, (size_t)ns * sizeof(wva_grid_best), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    const uint32_t qnan = WVA_BLOCK_NAN;
+    std::vector<unsigned long long> ids;
+    for (int sl = 0; sl < ns; ++sl) {
+        std::memcpy(&p_block[sl], &qnan, 4);
+        const wva_grid_best& w = best[(size_t)sl];
+        if (w.acc < 0) continue;
+        ids.push_back((((unsigned long long)sl * ctx->A + (unsigned)w.acc) * (unsigned)ctx->grid_r + (unsigned)(w.replicas - 1)) *
+                          (unsigned)ctx->grid_b + (unsigned)(w.batch - 1));
+    }
+    const int n = (int)ids.size();
+    if (n == 0) return WVA_OK;
+    // [n ids][ns floats]
+    CK(ctx->blkIo.ensure((size_t)n * 8 + (size_t)ns * 4));
+    unsigned long long* idsDev = ctx->blkIo.as<unsigned long long>();
+    float* outDev = reinterpret_cast<float*>(idsDev + n);
+    CK(ctx->blkCount.ensure(2 * 8));
+    CK(ctx->blkLit.ensure((size_t)n * 8));
+    ctx->blk_lit_n = 0;                              // the plane's literal list is overwritten (the plane is not)
+    CK(cudaMemcpyAsync(idsDev, ids.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(outDev, p_block, (size_t)ns * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(ctx->blkCount.as<unsigned long long>() + 1, 0, 8, ctx->stream));
+    const BlockParams bp = block_params(ctx);
+    int rc = block_finish(ctx, bp, idsDev, n, outDev, 1);
+    if (rc != WVA_OK) return rc;
+    CK(cudaMemcpyAsync(p_block, outDev, (size_t)ns * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     return WVA_OK;
 }
 
@@ -1791,6 +1973,11 @@ int wva_group_pairs_fetch(wva_group* g, wva_alloc_soa* out, uint8_t* feasible) {
 int wva_group_grid_fetch(wva_group* g, wva_grid_best* best) {
     if (!g || !best) return WVA_EINVAL;
     return g->each([&](int, wva_ctx* c) { return wva_grid_fetch(c, best + c->s0); });
+}
+
+int wva_group_grid_best_blocking(wva_group* g, float* p_block) {
+    if (!g || !p_block) return WVA_EINVAL;
+    return g->each([&](int, wva_ctx* c) { return wva_grid_best_blocking(c, p_block + c->s0); });
 }
 
 int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen) {
