@@ -886,9 +886,10 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
         CK(cudaFuncSetAttribute(k_scan_cert<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     CK(cudaFuncSetAttribute(k_grid_list_own, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    // k_grid_wrow: the table, then per warp the checkpoints and the quotient buffer of warp_exact
+    // k_grid_wrow: the table, then per warp the checkpoints and the quotient buffer of warp_exact.  Only set when it
+    // runs: above b_max ~ 7 500 smemW exceeds the SM's shared memory and the attribute call fails
     const size_t smemW = align_up(smem, 16) + (size_t)(WVA_GRID_THREADS / 32) * (WVA_WX_CP + 1 + 1024) * 8;
-    if (smemW > 48 * 1024) CK(cudaFuncSetAttribute(k_grid_wrow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemW));
+    if (wrowMode && smemW > 48 * 1024) CK(cudaFuncSetAttribute(k_grid_wrow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemW));
     if (slicePairsMax * (size_t)gp.n_rchunks > 0x7fffffffULL) return fail(ctx, WVA_EINVAL, "too many grid blocks");
     {
         const size_t perPairBlocks = (size_t)(gp.n_rchunks > gp.n_bseg ? gp.n_rchunks : gp.n_bseg);
