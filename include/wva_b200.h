@@ -488,18 +488,22 @@ void* wva_stream(const wva_ctx* ctx);
  * sent to the materialised-p[] path. */
 int wva_grid_set_tail_cap(wva_ctx* ctx, int32_t tail_cap);
 int wva_grid_list_sizes(const wva_ctx* ctx, int32_t* deferred, int32_t* literal);
-/* Tuning (sweep): when the previous sweep deferred more than 4096 candidates to the exact-chain kernels, the next one
- * launches all its kernels without stopping at the host in between (the chain kernel reads the list length from device
- * memory and runs on SMs of its own beside the cube-writing half).  on = 1 (default) / 0 = always stop and go.  Same
- * results either way.  wva_grid_last_fused: 1 when the last sweep slice ran that way. */
+/* Tuning (sweep): when the last sweep slice run on this context -- the previous slice of the same call, or the last
+ * slice of an earlier call, whatever was uploaded or sharded since -- deferred more than 4096 candidates to the
+ * exact-chain kernels, the next slice launches all its kernels without stopping at the host in between (the chain
+ * kernel reads the list length from device memory and runs on SMs of its own beside the cube-writing half).  Its list
+ * gets 2 * that length + 65536 slots; a slice whose list outgrows them is redone stop and go.  on = 1 (default) / 0 =
+ * always stop and go.  Same results either way.  wva_grid_last_fused: 1 when the last sweep slice ran that way. */
 int wva_grid_set_fused(wva_ctx* ctx, int32_t on);
 int wva_grid_last_fused(const wva_ctx* ctx);
 /* Candidate ids (cube indices relative to the shard) the last sweep slice handed to the exact-chain
  * kernel because their certificate was ambiguous or their tail outlasted tail_cap (at most cap are
  * copied; *n = how many there were).  Test/diagnostic aid: parity tests re-evaluate exactly these. */
 int wva_grid_deferred_fetch(wva_ctx* ctx, uint64_t* ids, int32_t cap, int32_t* n);
-/* Work counters of the last grid sweep: chain steps actually executed and the
- * algorithmic chain steps (sum over analysable candidates of 2*(11b+1)). */
+/* Work counters of the last grid sweep: chain steps actually executed, the algorithmic chain steps (sum over
+ * analysable candidates of 2*(11b+1)) and the analysable candidates.  A slice whose deferred or literal list outgrew
+ * its buffer is swept again; the algorithmic steps and the analysable candidates count each candidate once however
+ * often its slice ran, the executed steps count every step that ran, those of the discarded attempts included. */
 int wva_grid_counters(const wva_ctx* ctx, uint64_t* steps_executed, uint64_t* steps_algorithmic,
                       uint64_t* candidates_ok);
 

@@ -768,7 +768,7 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
     const size_t nCand = nPairs * perPair;
     CK(ctx->keys.ensure((size_t)(ns ? ns : 1) * 8));
     CK(ctx->bestDev.ensure((size_t)(ns ? ns : 1) * sizeof(wva_grid_best)));
-    CK(ctx->counters.ensure(3 * 8));
+    CK(ctx->counters.ensure(5 * 8));                  // [0..2] wva_grid_counters, [3..4] [1..2] as the current slice began
     CK(ctx->gridSlowCount.ensure(8));                 // [0] literal-path count, [1] deferred count
     CK(ctx->heavyHist.ensure(2 * 256 * 4));
     if (want_cube) {
@@ -929,6 +929,12 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
         // gets the others.  The list's slots are sized from the previous length; a list that outgrows them redoes the slice
         // the stop-and-go way (keys only ever decrease towards the true minimum: safe).
         bool fused = scanMode && ctx->grid_fused && ctx->heavy_hint > 4096;
+        // A slice that is redone counts its candidates once: the algorithmic steps and the analysed candidates go back to
+        // their values from before the slice (the executed steps keep counting the work that ran).  Called once every
+        // kernel of the attempt has finished, k_scan_lean included.
+        unsigned long long* const cnt = gp.counters;
+        CK(cudaMemcpyAsync(cnt + 3, cnt + 1, 2 * 8, cudaMemcpyDeviceToDevice, ctx->gstream));
+        auto undo_slice_counts = [&] { return cudaMemcpyAsync(cnt + 1, cnt + 3, 2 * 8, cudaMemcpyDeviceToDevice, ctx->gstream); };
         for (int attempt = 0; attempt < 3; ++attempt) {
             gp.slow_list = ctx->gridSlow.as<unsigned long long>(); gp.slow_cap = slow_cap;
             CK(cudaMemsetAsync(ctx->gridSlowCount.p, 0, 8, ctx->gstream));
@@ -977,6 +983,7 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
                 if ((size_t)counts[1] > fusedCap) {                    // the list outgrew its slots: once more, stop-and-go
                     ctx->heavy_hint = 0; fused = false;
                     CK(cudaStreamWaitEvent(ctx->gstream, ctx->evLean, 0));
+                    CK(undo_slice_counts());
                     continue;
                 }
                 heavy = counts[1];
@@ -984,6 +991,7 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
                 slow_cap = slow;
                 CK(ctx->gridSlow.ensure((size_t)slow_cap * 8));
                 CK(cudaStreamWaitEvent(ctx->gstream, ctx->evLean, 0));
+                CK(undo_slice_counts());
                 continue;
             }
             if (scanMode) {
@@ -1059,8 +1067,9 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
             if (slow <= slow_cap) break;
             slow_cap = slow;                          // rare: more literal-path candidates than the list holds
             CK(ctx->gridSlow.ensure((size_t)slow_cap * 8));
-            // keys only ever decrease towards the true minimum: redoing the slice is safe (the work
-            // counters then count the slice twice)
+            // keys only ever decrease towards the true minimum: redoing the slice is safe
+            if (leanPending) CK(cudaStreamWaitEvent(ctx->gstream, ctx->evLean, 0));
+            CK(undo_slice_counts());
         }
         ctx->last_heavy += heavy; ctx->last_slow += slow; ctx->last_heavy_slice = heavy; ctx->heavy_hint = heavy; ctx->last_fused = fused ? 1 : 0;
         int listSlots = heavy;

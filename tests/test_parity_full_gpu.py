@@ -81,15 +81,42 @@ def _check_sweep_against_oracle(wva, oracle, ctx, img, first, count, R, B, n_ran
     o_m, o_st = oracle.grid_candidates(img, s + first, a, r, b, threads=th)
     assert np.array_equal(o_st, status[idx.astype(np.int64)])
     assert o_m.tobytes() == cube[idx.astype(np.int64)].tobytes()
-    # (3) winners: own record ...
+    # (3) winners
+    (ls, la, lr), proof = prove_winners(wva, oracle, img, first + np.arange(count), best, R, B)
+    # the GPU's own feasibility flags agree with that (cheap cross-check of the status cube)
+    feas = (status & 1).reshape(count, A, R, B)
+    assert int(feas[ls, la, lr].sum()) == 0
+    ctx.set_shard(0, img.S)
+    return dict(candidates=ncand, checked=len(idx), deferred=int(n_def), winners=int((best["acc"] >= 0).sum()),
+                proof_candidates=proof, literal=lists["literal"])
+
+
+def _row_values(oracle, img, R, srv):
+    """oracle.grid_row_values of the listed servers, one call per run of consecutive ones -> [len(srv), A, R]"""
+    out = np.empty((len(srv), img.A, R), dtype=F)
+    for run in np.split(np.arange(len(srv)), np.flatnonzero(np.diff(srv) != 1) + 1):
+        s0 = int(srv[run[0]])
+        out[run] = oracle.grid_row_values(img, R, s0, s0 + len(run))
+    return out
+
+
+def prove_winners(wva, oracle, img, srv, best, R, B):
+    """The sweep records `best` of servers `srv` (indices into img) against the oracle: each winner's own record, and no
+    candidate with a smaller (value, a, r, b) key is feasible according to the oracle (a server without a winner has no
+    feasible candidate at all).  Returns the (server position, a, r - 1) of the rows that precede a winner as a whole,
+    and how many candidates the proof evaluated."""
+    th = _threads(oracle)
+    A = img.A
+    srv = np.asarray(srv, dtype=np.int64)
+    # own record ...
     has = best["acc"] >= 0
     ws = np.flatnonzero(has).astype(np.int32)
-    w_m, w_st = oracle.grid_candidates(img, ws + first, best["acc"][ws], best["replicas"][ws], best["batch"][ws], threads=th)
+    w_m, w_st = oracle.grid_candidates(img, srv[ws], best["acc"][ws], best["replicas"][ws], best["batch"][ws], threads=th)
     assert (w_st == (wva.abi.CAND_OK | wva.abi.CAND_FEASIBLE)).all()
     assert np.array_equal((w_m["avg_wait_time"] + w_m["avg_prefill_time"]).astype(F).view(np.uint32), best["ttft"][ws].view(np.uint32))
     assert np.array_equal(w_m["avg_token_time"].view(np.uint32), best["itl"][ws].view(np.uint32))
     assert np.array_equal(w_m["rho"].view(np.uint32), best["rho"][ws].view(np.uint32))
-    vals = oracle.grid_row_values(img, R, first, first + count)            # [count, A, R]
+    vals = _row_values(oracle, img, R, srv)                                # [len(srv), A, R]
     wv = vals[ws, best["acc"][ws], best["replicas"][ws] - 1]
     assert np.array_equal(wv.view(np.uint32), best["value"][ws].view(np.uint32))
     # ... and no candidate with a smaller (value, a, r, b) key is feasible according to the oracle
@@ -101,19 +128,14 @@ def _check_sweep_against_oracle(wva, oracle, ctx, img, first, count, R, B, n_ran
     with np.errstate(invalid="ignore"):
         lower = (vals < v_win) | ((vals == v_win) & (rowkey < k_win))      # NaN-valued rows are never selected
     ls, la, lr = np.nonzero(lower)
-    rows_s = np.concatenate([ls, ws]).astype(np.int32)
+    rows_s = np.concatenate([srv[ls], srv[ws]]).astype(np.int32)
     rows_a = np.concatenate([la, best["acc"][ws]]).astype(np.int32)
     rows_r = np.concatenate([lr + 1, best["replicas"][ws]]).astype(np.int32)
     b_lo = np.ones(len(rows_s), dtype=np.int32)
     b_hi = np.concatenate([np.full(len(ls), B), best["batch"][ws] - 1]).astype(np.int32)
-    nf = oracle.grid_rows_feasible(img, rows_s + first, rows_a, rows_r, b_lo, b_hi, threads=th)
+    nf = oracle.grid_rows_feasible(img, rows_s, rows_a, rows_r, b_lo, b_hi, threads=th)
     assert int(nf.sum()) == 0, "the oracle finds a feasible candidate that precedes a GPU winner"
-    # the GPU's own feasibility flags agree with that (cheap cross-check of the status cube)
-    feas = (status & 1).reshape(count, A, R, B)
-    assert int(feas[ls, la, lr].sum()) == 0
-    ctx.set_shard(0, img.S)
-    return dict(candidates=ncand, checked=len(idx), deferred=int(n_def), winners=int(has.sum()),
-                proof_candidates=int((b_hi - b_lo + 1).clip(min=0).sum()), literal=lists["literal"])
+    return (ls, la, lr), int((b_hi - b_lo + 1).clip(min=0).sum())
 
 
 def test_config3_sweep_vs_oracle(wva, oracle, ctx):
