@@ -284,6 +284,44 @@ func (c *Context) GridBestBlocking(s int) ([]float32, error) {
 	return out, c.err(C.wva_grid_best_blocking(c.ctx, f32p(out)), "wva_grid_best_blocking")
 }
 
+// PairRec is wva_pair_rec: one core.Allocation with its feasible flag, pointer-free (48 bytes, same layout as C).
+type PairRec struct {
+	Acc                    int32
+	Feasible               uint8
+	Pad                    [3]uint8
+	NumReplicas, BatchSize int64
+	Cost, Value, ITL, TTFT, Rho, MaxArrvRatePerReplica float32
+}
+
+func pairRecs(r []PairRec) *C.wva_pair_rec {
+	if len(r) == 0 {
+		return nil
+	}
+	return (*C.wva_pair_rec)(unsafe.Pointer(&r[0]))
+}
+
+// PairsAtBatchSizes sizes every pair of the shard under each ServerSpec.MaxBatchSize override of batches (strictly
+// increasing, values in 1..8192): plane[((srv-first)*A+a)*len(batches)+j] is CreateAllocation's record under batches[j]
+// (nil unless wantPlane), best[srv-first] is SolveUnlimited over the server's records.  The slices are sized from the
+// library's own shard and dimensions.  The resident pair records, decisions and sweep results are left as they were.
+func (c *Context) PairsAtBatchSizes(batches []int32, wantPlane bool) (plane, best []PairRec, err error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var S, A, M, T, first, count C.int32_t
+	if err = c.err(C.wva_system_dims(c.ctx, &S, &A, &M, &T), "wva_system_dims"); err != nil {
+		return nil, nil, err
+	}
+	if err = c.err(C.wva_shard_info(c.ctx, &first, &count), "wva_shard_info"); err != nil {
+		return nil, nil, err
+	}
+	best = make([]PairRec, int(count))
+	if wantPlane {
+		plane = make([]PairRec, int(count)*int(A)*len(batches))
+	}
+	return plane, best, c.err(C.wva_analyze_pairs_batches(c.ctx, C.int32_t(len(batches)), i32p(batches), pairRecs(plane), pairRecs(best)),
+		"wva_analyze_pairs_batches")
+}
+
 // QueueConfig is wva_queue_config; Metrics is wva_metrics (analyzer.AnalysisMetrics).
 type QueueConfig struct {
 	MaxBatchSize, MaxQueueSize int32
@@ -409,6 +447,22 @@ func (g *Group) GridBestBlocking(s int) ([]float32, error) {
 		return out, nil
 	}
 	return out, g.err(C.wva_group_grid_best_blocking(g.g, f32p(out)), "wva_group_grid_best_blocking")
+}
+
+// PairsAtBatchSizes: Context.PairsAtBatchSizes over every device's servers, assembled (sized from device 0's image).
+func (g *Group) PairsAtBatchSizes(batches []int32, wantPlane bool) (plane, best []PairRec, err error) {
+	g.mu.Lock()
+	defer g.mu.Unlock()
+	var S, A, M, T C.int32_t
+	if rc := C.wva_system_dims(C.wva_group_ctx(g.g, 0), &S, &A, &M, &T); rc != C.WVA_OK {
+		return nil, nil, fmt.Errorf("wva_system_dims: %d", int(rc))
+	}
+	best = make([]PairRec, int(S))
+	if wantPlane {
+		plane = make([]PairRec, int(S)*int(A)*len(batches))
+	}
+	return plane, best, g.err(C.wva_group_analyze_pairs_batches(g.g, C.int32_t(len(batches)), i32p(batches), pairRecs(plane), pairRecs(best)),
+		"wva_group_analyze_pairs_batches")
 }
 
 // AllocateByType: global per-type totals (NCCL all-gather of the partials inside the library).

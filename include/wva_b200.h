@@ -231,6 +231,8 @@ int wva_solve_arrays(wva_ctx* ctx, int32_t unlimited, int32_t delayed_best_effor
  * uploaded image; analysis kernels touch only those; solve/allocate_by_type produce the
  * rank's partial results.  Default shard = everything. */
 int wva_set_shard(wva_ctx* ctx, int32_t first_server, int32_t count);
+/* The shard the following calls work on: servers [*first, *first + *count).  WVA_ESTATE before any upload. */
+int wva_shard_info(const wva_ctx* ctx, int32_t* first, int32_t* count);
 
 /* ---- Analyze ------------------------------------------------------------- */
 
@@ -338,6 +340,36 @@ int wva_pair_counters(wva_ctx* ctx, uint64_t out[4]);
  * (bits 36-43) | chain steps / 1024 (bits 44-63); [1] = (rounds << 32) | rounds-with-evaluations. */
 int wva_pair_debug(wva_ctx* ctx, uint64_t* out, int32_t n_pairs);
 
+/* One core.Allocation with its feasible flag, pointer-free so that cgo can pass slices of it. */
+typedef struct wva_pair_rec {
+    int32_t acc;            /* accelerator index; WVA_ACC_NONE in the empty record */
+    uint8_t feasible;       /* 1 when CreateAllocation returned non-nil and the accelerator is a candidate */
+    uint8_t pad[3];         /* always 0 */
+    int64_t num_replicas, batch_size;
+    float   cost, value, itl, ttft, rho, max_arrv_rate_per_replica;
+} wva_pair_rec;             /* 48 bytes */
+
+/* Pair sizing over a list of batch-size overrides.  batch[0..n_b) is strictly increasing, 1 <= n_b <= 8192, each value
+ * in 1..8192.  Record (s, a, j) is the record wva_pairs_fetch gives for pair (s, a) after uploading the same image with
+ * srv_max_batch[s] = batch[j] for every server (ServerSpec.MaxBatchSize = batch[j]; the server's own override is
+ * replaced): candidate filter, CreateAllocation (allocation.go:27-163, zero-load servers included: their batch is
+ * batch[j]), value = TransitionPenalty, the empty record with feasible = 0 where CreateAllocation returns nil.
+ *   plane [servers of the shard * A * n_b], index ((s - s0) * A + a) * n_b + j, or NULL (not copied to the host);
+ *   best  [servers of the shard], or NULL: SolveUnlimited (pkg/solver/solver.go:63-79) over each server's A * n_b
+ *         records -- the first feasible record, in order of a then j, whose value is strictly below every earlier one
+ *         starting from MaxFloat32 (NaN, +Inf and MaxFloat32 itself are never chosen; -0 and +0 tie); the empty record
+ *         (acc = -1, feasible = 0) when there is none.
+ * The records are staged in HBM in slices of at most 2^28 bytes of servers (one server at least) and each slice is
+ * copied out before the next starts.  Nothing that other calls read changes: pair records, decisions, totals and
+ * sweep results, and whether they are valid, stay as they were.  WVA_EINVAL for a bad list, WVA_ESTATE before any
+ * upload. */
+#define WVA_PAIRS_MAX_BATCH   8192
+#define WVA_PAIRS_MAX_BATCHES 8192
+int wva_analyze_pairs_batches(wva_ctx* ctx, int32_t n_b, const int32_t* batch, wva_pair_rec* plane, wva_pair_rec* best);
+/* Counters of the last wva_analyze_pairs_batches: {server slices, items (pair, batch size) sent to the materialised-p[]
+ * path, chain steps executed, items sized (those that reached the queue analyzer)}. */
+int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]);
+
 /* ---- Optimize ------------------------------------------------------------ */
 
 /* Replaces solver.Solver.Solve (pkg/solver/solver.go:32-60): SolveUnlimited (:63-79) or
@@ -432,6 +464,8 @@ int wva_group_analyze(wva_group* g, int32_t r_max, int32_t b_max, int32_t want_c
 int wva_group_pairs_fetch(wva_group* g, wva_alloc_soa* out, uint8_t* feasible);
 int wva_group_grid_fetch(wva_group* g, wva_grid_best* best /* [S] */);
 int wva_group_grid_best_blocking(wva_group* g, float* p_block /* [S] */);   /* wva_grid_best_blocking, assembled */
+int wva_group_analyze_pairs_batches(wva_group* g, int32_t n_b, const int32_t* batch,
+                                    wva_pair_rec* plane /* [S*A*n_b] */, wva_pair_rec* best /* [S] */);   /* assembled */
 int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen);
 int wva_group_allocate_by_type(wva_group* g, int64_t* count, float* cost);
 

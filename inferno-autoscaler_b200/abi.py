@@ -111,6 +111,21 @@ QUEUE_CONFIG_DTYPE = np.dtype([("max_batch_size", "<i4"), ("max_queue_size", "<i
                                ("beta", "<f4"), ("gamma", "<f4"), ("delta", "<f4"),
                                ("avg_input_tokens", "<i4"), ("avg_output_tokens", "<i4")])
 
+class PairRec(C.Structure):
+    _fields_ = [("acc", C.c_int32), ("feasible", C.c_uint8), ("pad", C.c_uint8 * 3), ("num_replicas", C.c_int64),
+                ("batch_size", C.c_int64), ("cost", C.c_float), ("value", C.c_float), ("itl", C.c_float),
+                ("ttft", C.c_float), ("rho", C.c_float), ("max_arrv_rate_per_replica", C.c_float)]
+
+
+# wva_pair_rec: one core.Allocation of wva_analyze_pairs_batches (explicit offsets: the C struct's padding)
+PAIR_REC_DTYPE = np.dtype(dict(
+    names=["acc", "feasible", "pad", "num_replicas", "batch_size", "cost", "value", "itl", "ttft", "rho",
+           "max_arrv_rate_per_replica"],
+    formats=["<i4", "u1", ("u1", 3), "<i8", "<i8", "<f4", "<f4", "<f4", "<f4", "<f4", "<f4"],
+    offsets=[0, 4, 5, 8, 16, 24, 28, 32, 36, 40, 44], itemsize=48))
+PAIRS_MAX_BATCH = PAIRS_MAX_BATCHES = 8192
+
+assert C.sizeof(PairRec) == PAIR_REC_DTYPE.itemsize == 48
 assert C.sizeof(Metrics) == METRICS_DTYPE.itemsize == 32
 assert C.sizeof(GridBest) == GRID_BEST_DTYPE.itemsize == 32
 assert C.sizeof(QueueConfig) == QUEUE_CONFIG_DTYPE.itemsize == 32

@@ -31,6 +31,7 @@ EXPORTS = [
     "wva_group_analyze", "wva_group_pairs_fetch", "wva_group_grid_fetch", "wva_group_solve", "wva_group_allocate_by_type",
     "wva_grid_blocking", "wva_grid_blocking_size", "wva_grid_blocking_device", "wva_grid_best_blocking", "wva_grid_blocking_counts", "wva_grid_blocking_exact_fetch",
     "wva_group_grid_best_blocking",
+    "wva_analyze_pairs_batches", "wva_pairs_batches_counters", "wva_group_analyze_pairs_batches", "wva_shard_info",
 ]
 
 
@@ -131,6 +132,10 @@ def lib():
         L.wva_grid_blocking_counts.argtypes = [vp, abi.i64p]
         L.wva_grid_blocking_exact_fetch.argtypes = [vp, C.POINTER(u64), i32, C.POINTER(i32)]
         L.wva_group_grid_best_blocking.argtypes = [vp, abi.f32p]
+        L.wva_analyze_pairs_batches.argtypes = [vp, i32, abi.i32p, vp, vp]
+        L.wva_pairs_batches_counters.argtypes = [vp, C.POINTER(u64)]
+        L.wva_group_analyze_pairs_batches.argtypes = [vp, i32, abi.i32p, vp, vp]
+        L.wva_shard_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
         if L.wva_abi_version() != abi.ABI_VERSION:
             raise ImportError("libwva_b200.so ABI version mismatch")
         _lib = L
@@ -285,6 +290,24 @@ class Context:
         feasible = np.zeros(n, dtype=np.uint8)
         self._ck(lib().wva_pairs_fetch(self._h, C.byref(out.c), abi.ptr(feasible, C.c_uint8)))
         return out, feasible
+
+    def analyze_pairs_batches(self, batch, plane=True):
+        """Pair sizing under each batch-size override of `batch` (strictly increasing, values in 1..8192): returns
+        (plane, best), numpy arrays of abi.PAIR_REC_DTYPE.  plane[(s - first) * A + a, j] is the record of pair (s, a)
+        with ServerSpec.MaxBatchSize = batch[j], or None when plane=False (it then stays off PCIe); best[s - first] is
+        SolveUnlimited over the server's records.  Resident results are left as they were."""
+        b = np.ascontiguousarray(batch, dtype=np.int32)
+        best = np.zeros(self.count, dtype=abi.PAIR_REC_DTYPE)
+        pl = np.zeros((self.count * self.image.A, len(b)), dtype=abi.PAIR_REC_DTYPE) if plane else None
+        self._ck(lib().wva_analyze_pairs_batches(self._h, len(b), abi.ptr(b, C.c_int32),
+                                                 pl.ctypes.data if plane else None, best.ctypes.data))
+        return pl, best
+
+    def pairs_batches_counters(self):
+        """counters of the last analyze_pairs_batches"""
+        v = (C.c_uint64 * 4)()
+        self._ck(lib().wva_pairs_batches_counters(self._h, v))
+        return dict(slices=v[0], materialised=v[1], steps=v[2], sized=v[3])
 
     def pair_counters(self):
         v = (C.c_uint64 * 4)()
@@ -572,6 +595,15 @@ class Group:
         out = np.empty(self.image.S, dtype=np.float32)
         self._ck(lib().wva_group_grid_best_blocking(self._h, abi.ptr(out, C.c_float)))
         return out
+
+    def analyze_pairs_batches(self, batch, plane=True):
+        """Context.analyze_pairs_batches over every device's servers, assembled: plane [S * A, n_b], best [S]"""
+        b = np.ascontiguousarray(batch, dtype=np.int32)
+        best = np.zeros(self.image.S, dtype=abi.PAIR_REC_DTYPE)
+        pl = np.zeros((self.image.S * self.image.A, len(b)), dtype=abi.PAIR_REC_DTYPE) if plane else None
+        self._ck(lib().wva_group_analyze_pairs_batches(self._h, len(b), abi.ptr(b, C.c_int32),
+                                                       pl.ctypes.data if plane else None, best.ctypes.data))
+        return pl, best
 
     def solve(self, unlimited=True, delayed_best_effort=False, policy=abi.POLICY_NONE, download=True):
         spec = abi.OptimizerSpec(1 if unlimited else 0, 1 if delayed_best_effort else 0, int(policy))

@@ -188,6 +188,9 @@ struct wva_ctx {
     int grid_scan = 1;          // certified sweeps: 1 = the scan kernels k_scan_prep / k_scan_cert / k_scan_lean (default), 0 = the round-1 kernels
     int pairs_debug = 0;
     DevBuf pairDbg;
+    // wva_analyze_pairs_batches: buffers of its own, so the resident pair results above stay as they are
+    DevBuf pbBatch, pbSlow, pbScratch, pbScratchOff, pbPlane, pbBest, pbCount;
+    uint64_t pb_counters[4] = {0, 0, 0, 0};
 
     // solution
     DevBuf chosenBuf; DevAllocs chosen{}; int* chosen_acc = nullptr; bool solved = false;
@@ -402,7 +405,9 @@ void wva_ctx_destroy(wva_ctx* ctx) {
                       &ctx->gridSlow, &ctx->gridSlowCount, &ctx->faultList, &ctx->faultCount, &ctx->heavyList, &ctx->heavyCost,
                       &ctx->heavyOrder, &ctx->heavyHist, &ctx->pairTab, &ctx->blockSlot, &ctx->listSlot, &ctx->gscratch, &ctx->rowInfo, &ctx->rateTab, &ctx->ioA, &ctx->ioB,
                       &ctx->ioC, &ctx->ioD, &ctx->ioE, &ctx->ioF, &ctx->ioG, &ctx->commTotals, &ctx->commChunk, &ctx->commGather,
-                      &ctx->blkPlane, &ctx->blkExact, &ctx->blkLit, &ctx->blkCount, &ctx->blkCounts, &ctx->blkScratch, &ctx->blkIo};
+                      &ctx->blkPlane, &ctx->blkExact, &ctx->blkLit, &ctx->blkCount, &ctx->blkCounts, &ctx->blkScratch, &ctx->blkIo,
+                      &ctx->pbBatch, &ctx->pbSlow, &ctx->pbScratch, &ctx->pbScratchOff,
+                      &ctx->pbPlane, &ctx->pbBest, &ctx->pbCount};
     for (DevBuf* b : bufs) b->release();
     ctx->staging.release();
     cudaEventDestroy(ctx->ev0);
@@ -752,6 +757,101 @@ int wva_pair_counters(wva_ctx* ctx, uint64_t out[4]) {
     if (!ctx->stepCounter.p) { out[0] = out[1] = out[2] = out[3] = 0; return WVA_OK; }
     CK(cudaSetDevice(ctx->device));
     CK(cudaMemcpy(out, ctx->stepCounter.p, 32, cudaMemcpyDeviceToHost));
+    return WVA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Pair sizing over a list of batch sizes.  Per slice of servers, k_pairs_plane sizes every (pair, b) item into the
+// slice's plane, k_pairs_plane_literal re-runs the items it sent to the materialised path, k_pairs_plane_best picks each
+// server's record, and the slice is copied out before the next one starts.  Buffers of its own: the resident pair
+// results stay as they are.
+int wva_analyze_pairs_batches(wva_ctx* ctx, int32_t n_b, const int32_t* batch, wva_pair_rec* plane, wva_pair_rec* best) {
+    if (!ctx) return WVA_EINVAL;
+    if (n_b < 1 || n_b > WVA_PAIRS_MAX_BATCHES || !batch) return fail(ctx, WVA_EINVAL, "batch list: 1 <= n_b <= 8192 values required");
+    for (int j = 0; j < n_b; ++j) {
+        if (batch[j] < 1 || batch[j] > WVA_PAIRS_MAX_BATCH) return fail(ctx, WVA_EINVAL, "batch sizes must lie in 1..8192");
+        if (j > 0 && batch[j] <= batch[j - 1]) return fail(ctx, WVA_EINVAL, "batch sizes must be strictly increasing");
+    }
+    if (!ctx->have_system) return fail(ctx, WVA_ESTATE, "no system uploaded");
+    const int A = ctx->A, ns = ctx->ns;
+    const size_t perServer = (size_t)A * (size_t)n_b;
+    if (perServer > 0x7fffffffULL) return fail(ctx, WVA_EINVAL, "A * n_b exceeds 2^31-1");
+    CK(cudaSetDevice(ctx->device));
+    for (int k = 0; k < 4; ++k) ctx->pb_counters[k] = 0;
+    if (ns == 0) return WVA_OK;
+    const size_t recBytes = perServer * sizeof(wva_pair_rec);
+    const int slice = (int)std::max<size_t>(1, std::min<size_t>((size_t)ns, ((size_t)1 << 28) / recBytes));
+    const size_t maxItems = (size_t)slice * perServer;
+    CK(ctx->pbBatch.ensure((size_t)n_b * 4));
+    CK(ctx->pbSlow.ensure(maxItems * 8));
+    CK(ctx->pbPlane.ensure((size_t)slice * recBytes));
+    CK(ctx->pbBest.ensure((size_t)slice * sizeof(wva_pair_rec)));
+    CK(ctx->pbCount.ensure(64));
+    // [0, 4) slow-list length, [8, 48) k_pairs_plane's counters
+    char* cnt = ctx->pbCount.as<char>();
+    int* slowCount = reinterpret_cast<int*>(cnt);
+    unsigned long long* counters = reinterpret_cast<unsigned long long*>(cnt + 8);
+    CK(cudaMemsetAsync(cnt, 0, 64, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->pbBatch.p, batch, (size_t)n_b * 4, cudaMemcpyHostToDevice, ctx->stream));
+    const int* dBatch = ctx->pbBatch.as<int>();
+    wva_pair_rec* dPlane = ctx->pbPlane.as<wva_pair_rec>();
+    wva_pair_rec* dBest = ctx->pbBest.as<wva_pair_rec>();
+    unsigned long long* dSlow = ctx->pbSlow.as<unsigned long long>();
+    const size_t smemBytes = (size_t)batch[n_b - 1] * 16;        // the table up to the largest b: at most 128 KB
+    if (smemBytes > 48 * 1024) CK(cudaFuncSetAttribute(k_pairs_plane, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+    std::vector<unsigned long long> items;
+    std::vector<long long> offs;
+    uint64_t nSlices = 0, nSlow = 0;
+    for (int f = ctx->s0; f < ctx->s0 + ns; f += slice) {
+        const int nss = std::min(slice, ctx->s0 + ns - f);
+        const int nPairs = nss * A;
+        CK(cudaMemsetAsync(slowCount, 0, 4, ctx->stream));
+        k_pairs_plane<<<nPairs, WVA_PAIRS_WARP_THREADS, smemBytes, ctx->stream>>>(ctx->dsys, f, dBatch, n_b, dPlane, dSlow, slowCount,
+                                                                                  counters);
+        LAUNCH_CHECK();
+        int slow = 0;
+        CK(cudaMemcpyAsync(&slow, slowCount, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (slow > 0) {
+            // items whose chain hit an overflow-rescale branch or whose table prefix holds an unusable entry: p[] in HBM
+            items.resize((size_t)slow);
+            offs.resize((size_t)slow);
+            CK(cudaMemcpy(items.data(), dSlow, (size_t)slow * 8, cudaMemcpyDeviceToHost));
+            long long total = 0;
+            for (int i = 0; i < slow; ++i) { offs[(size_t)i] = total; total += 11LL * batch[items[(size_t)i] % (unsigned)n_b] + 1; }
+            size_t freeB = 0, totB = 0;
+            CK(cudaMemGetInfo(&freeB, &totB));
+            if ((size_t)total * 8 > freeB / 2) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
+            CK(ctx->pbScratch.ensure((size_t)total * 8));
+            CK(ctx->pbScratchOff.ensure((size_t)slow * 8));
+            CK(cudaMemcpyAsync(ctx->pbScratchOff.p, offs.data(), (size_t)slow * 8, cudaMemcpyHostToDevice, ctx->stream));
+            k_pairs_plane_literal<<<(slow + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, dBatch, n_b, dSlow, slow, ctx->pbScratch.as<double>(),
+                                                                           ctx->pbScratchOff.as<long long>(), dPlane, counters);
+            LAUNCH_CHECK();
+            nSlow += (uint64_t)slow;
+        }
+        k_pairs_plane_best<<<(nss + 3) / 4, 128, 0, ctx->stream>>>(dPlane, nss, (int)perServer, dBest);
+        LAUNCH_CHECK();
+        const size_t hs = (size_t)(f - ctx->s0);
+        if (plane) CK(cudaMemcpyAsync(plane + hs * perServer, dPlane, (size_t)nss * recBytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (best) CK(cudaMemcpyAsync(best + hs, dBest, (size_t)nss * sizeof(wva_pair_rec), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));       // also releases offs for the next slice
+        ++nSlices;
+    }
+    unsigned long long dev[5];
+    CK(cudaMemcpy(dev, counters, sizeof dev, cudaMemcpyDeviceToHost));
+    ctx->pb_counters[0] = nSlices; ctx->pb_counters[1] = nSlow; ctx->pb_counters[2] = dev[0]; ctx->pb_counters[3] = dev[4];
+    return WVA_OK;
+}
+int wva_shard_info(const wva_ctx* ctx, int32_t* first, int32_t* count) {
+    if (!ctx || !first || !count) return WVA_EINVAL;
+    if (!ctx->have_system) return WVA_ESTATE;
+    *first = ctx->s0; *count = ctx->ns;
+    return WVA_OK;
+}
+int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]) {
+    if (!ctx || !out) return WVA_EINVAL;
+    for (int k = 0; k < 4; ++k) out[k] = ctx->pb_counters[k];
     return WVA_OK;
 }
 
@@ -1988,6 +2088,15 @@ int wva_group_grid_fetch(wva_group* g, wva_grid_best* best) {
 int wva_group_grid_best_blocking(wva_group* g, float* p_block) {
     if (!g || !p_block) return WVA_EINVAL;
     return g->each([&](int, wva_ctx* c) { return wva_grid_best_blocking(c, p_block + c->s0); });
+}
+
+int wva_group_analyze_pairs_batches(wva_group* g, int32_t n_b, const int32_t* batch, wva_pair_rec* plane, wva_pair_rec* best) {
+    if (!g) return WVA_EINVAL;
+    const bool okList = n_b >= 1 && n_b <= WVA_PAIRS_MAX_BATCHES;    // otherwise every device fails with WVA_EINVAL
+    return g->each([&](int, wva_ctx* c) {
+        wva_pair_rec* p = (plane && okList) ? plane + (size_t)c->s0 * (size_t)c->A * (size_t)n_b : nullptr;
+        return wva_analyze_pairs_batches(c, n_b, batch, p, best ? best + c->s0 : nullptr);
+    });
 }
 
 int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen) {

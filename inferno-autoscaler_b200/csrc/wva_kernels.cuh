@@ -68,15 +68,15 @@ __device__ __forceinline__ bool is_candidate_accel(const DevSystem& sys, int s, 
     return true;
 }
 
-// zeroLoadAllocation, allocation.go:259-288
-__device__ AllocRec zero_load_allocation(const DevSystem& sys, int s, int a) {
+// zeroLoadAllocation, allocation.go:259-288, under ServerSpec.MaxBatchSize = over (0 = none)
+__device__ AllocRec zero_load_allocation_n(const DevSystem& sys, int s, int a, long long over) {
     AllocRec out = empty_alloc();
     long long numReplicas = sys.srv_min_replicas[s];
     if (numReplicas == 0) return out;
     int m = sys.srv_model[s];
     size_t pi = (size_t)m * sys.A + a;
     long long maxBatch = sys.perf_max_batch[pi];
-    if (sys.srv_max_batch[s] > 0) maxBatch = sys.srv_max_batch[s];
+    if (over > 0) maxBatch = over;
     long long total = go_muli(num_instances(sys, m, a), numReplicas);
     float cost = sys.acc_cost[a] * (float)total;
     float alpha = sys.perf_alpha[pi], beta = sys.perf_beta[pi], gamma = sys.perf_gamma[pi], delta = sys.perf_delta[pi];
@@ -90,6 +90,9 @@ __device__ AllocRec zero_load_allocation(const DevSystem& sys, int s, int a) {
     out.maxArrv = (float)maxBatch / maxServ;
     out.value = cost;
     return out;
+}
+__device__ __forceinline__ AllocRec zero_load_allocation(const DevSystem& sys, int s, int a) {
+    return zero_load_allocation_n(sys, s, a, sys.srv_max_batch[s]);
 }
 
 // N of CreateAllocation (allocation.go:77-87); 0 when the pair never reaches the queue analyzer.
@@ -105,18 +108,18 @@ __device__ __forceinline__ long long pair_batch_size(const DevSystem& sys, int s
 // core.CreateAllocation, allocation.go:27-163.  Returns false for nil.  `fault` is set when the
 // streaming solver met an overflow-rescale case and no scratch was supplied (caller re-runs the
 // pair in the literal kernel).
-__device__ bool create_allocation(const DevSystem& sys, int s, int a, double* scratch, AllocRec& out, int& fault,
-                                  unsigned long long& steps) {
+__device__ bool create_allocation_n(const DevSystem& sys, int s, int a, long long over, double* scratch, AllocRec& out,
+                                    int& fault, unsigned long long& steps) {
     fault = 0;
     if (!pair_lookups_ok(sys, s, a)) return false;
     const float arrival = sys.srv_arrival_rpm[s];
     const long long inTok = sys.srv_in_tokens[s], outTok = sys.srv_out_tokens[s];
-    if (arrival == 0.0f || outTok == 0) { out = zero_load_allocation(sys, s, a); return true; }
+    if (arrival == 0.0f || outTok == 0) { out = zero_load_allocation_n(sys, s, a, over); return true; }
     const int m = sys.srv_model[s];
     const size_t pi = (size_t)m * sys.A + a;
     const long long K = outTok;
     long long N;
-    if (sys.srv_max_batch[s] > 0) N = sys.srv_max_batch[s];
+    if (over > 0) N = over;
     else { N = go_divi(go_muli(sys.perf_max_batch[pi], sys.perf_at_tokens[pi]), K); if (N < 1) N = 1; }
     const long long maxQueue = go_muli(N, WVA_MAX_QUEUE_TO_BATCH_RATIO);
     if (!config_ok(N, maxQueue, inTok, K)) return false;
@@ -152,15 +155,25 @@ __device__ bool create_allocation(const DevSystem& sys, int s, int a, double* sc
     return true;
 }
 
-// Server.Calculate for one pair: candidate filter + CreateAllocation + transition penalty (server.go:55-67)
-__device__ bool calculate_pair(const DevSystem& sys, int s, int a, double* scratch, AllocRec& out, int& fault,
-                               unsigned long long& steps) {
+__device__ __forceinline__ bool create_allocation(const DevSystem& sys, int s, int a, double* scratch, AllocRec& out, int& fault,
+                                                  unsigned long long& steps) {
+    return create_allocation_n(sys, s, a, sys.srv_max_batch[s], scratch, out, fault, steps);
+}
+
+// Server.Calculate for one pair: candidate filter + CreateAllocation + transition penalty (server.go:55-67), under
+// ServerSpec.MaxBatchSize = over
+__device__ bool calculate_pair_n(const DevSystem& sys, int s, int a, long long over, double* scratch, AllocRec& out, int& fault,
+                                 unsigned long long& steps) {
     fault = 0;
     if (!is_candidate_accel(sys, s, a)) return false;
-    if (!create_allocation(sys, s, a, scratch, out, fault, steps)) return false;
+    if (!create_allocation_n(sys, s, a, over, scratch, out, fault, steps)) return false;
     out.value = transition_penalty(sys.srv_cur_acc[s], sys.srv_cur_replicas[s], sys.srv_cur_cost[s], out.acc,
                                    out.numReplicas, out.cost);
     return true;
+}
+__device__ __forceinline__ bool calculate_pair(const DevSystem& sys, int s, int a, double* scratch, AllocRec& out, int& fault,
+                                               unsigned long long& steps) {
+    return calculate_pair_n(sys, s, a, sys.srv_max_batch[s], scratch, out, fault, steps);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -300,40 +313,29 @@ __device__ __forceinline__ SolveStats shfl_stats(const SolveStats& s, int src) {
     return o;
 }
 
-#define WVA_PAIRS_WARP_THREADS 128
-__global__ void __launch_bounds__(WVA_PAIRS_WARP_THREADS)
-k_pairs_warp(DevSystem sys, int s0, int nPairs, const long long* __restrict__ tabOff, double2* tabs, DevAllocs out,
-             unsigned char* feasible, int* slow_list, int* slow_count, unsigned long long* step_counter,
-             int smemEntriesPerWarp, double* pbuf, long long pbufStrideK, unsigned long long* dbg) {
-    extern __shared__ __align__(16) unsigned char pairs_smem[];
-    const long long tStart = clock64();
-    int activeRounds = 0, totalRounds = 0, pendEvals = 0;
-    long long solveCycles = 0;
-    const int pid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;      // warp-uniform
-    const int lane = threadIdx.x & 31;
-    if (pid >= nPairs) return;
-    const int s = s0 + pid / sys.A, a = pid % sys.A;
-    const size_t gi = (size_t)s * sys.A + a;
-    unsigned long long steps = 0;
-    AllocRec rec = empty_alloc();
-    bool ok = false;          // CreateAllocation != nil
-    bool toSlow = false;      // needs the materialised path (whole pair re-done by k_pairs_literal)
-
+// The body of k_pairs_warp for one pair under ServerSpec.MaxBatchSize = over (0 = none): candidate filter,
+// CreateAllocation by the warp (without the transition penalty).  table(wp, N) hands out the pair's {rate, reciprocal}
+// table of N entries, ready for use, or nullptr when the item must go to the materialised path.  Called by the 32 lanes
+// of a warp together.
+template <class Table>
+__device__ __forceinline__ void size_pair_warp(const DevSystem& sys, int s, int a, long long over, Table table, int lane,
+                                               unsigned long long* step_counter, AllocRec& rec, bool& ok, bool& toSlow,
+                                               unsigned long long& steps, int& activeRounds, int& totalRounds, int& pendEvals,
+                                               long long& solveCycles) {
     // every lane runs the scalar part redundantly (uniform control flow)
     do {
         if (!is_candidate_accel(sys, s, a) || !pair_lookups_ok(sys, s, a)) break;
         const float arrival = sys.srv_arrival_rpm[s];
         const long long inTok = sys.srv_in_tokens[s], outTok = sys.srv_out_tokens[s];
-        if (arrival == 0.0f || outTok == 0) { rec = zero_load_allocation(sys, s, a); ok = true; break; }
+        if (arrival == 0.0f || outTok == 0) { rec = zero_load_allocation_n(sys, s, a, over); ok = true; break; }
         const int m = sys.srv_model[s];
         const size_t pi = (size_t)m * sys.A + a;
         const long long Kt = outTok;
         long long N;
-        if (sys.srv_max_batch[s] > 0) N = sys.srv_max_batch[s];
+        if (over > 0) N = over;
         else { N = go_divi(go_muli(sys.perf_max_batch[pi], sys.perf_at_tokens[pi]), Kt); if (N < 1) N = 1; }
         const long long maxQueue = go_muli(N, WVA_MAX_QUEUE_TO_BATCH_RATIO);
         if (!config_ok(N, maxQueue, inTok, Kt)) break;
-        if (tabOff[pid] < 0 || N > (1LL << 26)) { toSlow = true; break; }   // no table budget: thread kernel handles it
         WarpPair wp;
         ServiceParms sp; sp.alpha = sys.perf_alpha[pi]; sp.beta = sys.perf_beta[pi];
         sp.gamma = sys.perf_gamma[pi]; sp.delta = sys.perf_delta[pi];
@@ -341,21 +343,8 @@ k_pairs_warp(DevSystem sys, int s0, int nPairs, const long long* __restrict__ ta
         wp.N = (int)N; wp.K = (int)(maxQueue + N); wp.inTok = inTok; wp.outTok = Kt;
         wp.tame = tame_parms(sp, inTok, Kt);
         wp.cert = sys.cert != 0;
-        // the table lives in shared memory when it fits (29-cycle loads in the ramp), else in HBM
-        double2* tab = (wp.N <= smemEntriesPerWarp)
-                           ? reinterpret_cast<double2*>(pairs_smem) + (size_t)(threadIdx.x >> 5) * smemEntriesPerWarp
-                           : tabs + tabOff[pid];
-        wp.pstore = (pbuf && (long long)wp.K + 1 <= pbufStrideK) ? pbuf + (size_t)pid * (size_t)pbufStrideK * 32 + lane : nullptr;
-        // BuildModel (queueanalyzer.go:99-131): the table, cooperatively
-        bool bad = false;
-        for (int i = lane; i < wp.N; i += 32) {
-            float r = wp.sv.rate(i + 1);
-            if (!(r > 0.0f) || !(r < CUDART_INF_F)) bad = true;
-            double d = (double)r;
-            tab[i] = make_double2(d, rcp_refined(d));
-        }
-        __syncwarp();
-        if (__any_sync(0xffffffffu, bad)) { toSlow = true; break; }
+        double2* tab = table(wp, N);           // nullptr: the item needs the materialised path
+        if (!tab) { toSlow = true; break; }
         wp.pv.tab = tab; wp.pv.sf = &wp.sv;
         {
             float lambdaMin = wp.sv.rate(1) * WVA_EPSILON;
@@ -542,6 +531,47 @@ k_pairs_warp(DevSystem sys, int s0, int nPairs, const long long* __restrict__ ta
         rec.value = cost;
         ok = true;
     } while (false);
+}
+
+#define WVA_PAIRS_WARP_THREADS 128
+__global__ void __launch_bounds__(WVA_PAIRS_WARP_THREADS)
+k_pairs_warp(DevSystem sys, int s0, int nPairs, const long long* __restrict__ tabOff, double2* tabs, DevAllocs out,
+             unsigned char* feasible, int* slow_list, int* slow_count, unsigned long long* step_counter,
+             int smemEntriesPerWarp, double* pbuf, long long pbufStrideK, unsigned long long* dbg) {
+    extern __shared__ __align__(16) unsigned char pairs_smem[];
+    const long long tStart = clock64();
+    int activeRounds = 0, totalRounds = 0, pendEvals = 0;
+    long long solveCycles = 0;
+    const int pid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;      // warp-uniform
+    const int lane = threadIdx.x & 31;
+    if (pid >= nPairs) return;
+    const int s = s0 + pid / sys.A, a = pid % sys.A;
+    const size_t gi = (size_t)s * sys.A + a;
+    unsigned long long steps = 0;
+    AllocRec rec = empty_alloc();
+    bool ok = false;          // CreateAllocation != nil
+    bool toSlow = false;      // needs the materialised path (whole pair re-done by k_pairs_literal)
+
+    auto table = [&](WarpPair& wp, long long N) -> double2* {
+        if (tabOff[pid] < 0 || N > (1LL << 26)) return nullptr;   // no table budget: thread kernel handles it
+        // the table lives in shared memory when it fits (29-cycle loads in the ramp), else in HBM
+        double2* tab = (wp.N <= smemEntriesPerWarp)
+                           ? reinterpret_cast<double2*>(pairs_smem) + (size_t)(threadIdx.x >> 5) * smemEntriesPerWarp
+                           : tabs + tabOff[pid];
+        wp.pstore = (pbuf && (long long)wp.K + 1 <= pbufStrideK) ? pbuf + (size_t)pid * (size_t)pbufStrideK * 32 + lane : nullptr;
+        // BuildModel (queueanalyzer.go:99-131): the table, cooperatively
+        bool bad = false;
+        for (int i = lane; i < wp.N; i += 32) {
+            float r = wp.sv.rate(i + 1);
+            if (!(r > 0.0f) || !(r < CUDART_INF_F)) bad = true;
+            double d = (double)r;
+            tab[i] = make_double2(d, rcp_refined(d));
+        }
+        __syncwarp();
+        return __any_sync(0xffffffffu, bad) ? nullptr : tab;
+    };
+    size_pair_warp(sys, s, a, sys.srv_max_batch[s], table, lane, step_counter, rec, ok, toSlow, steps, activeRounds, totalRounds,
+                   pendEvals, solveCycles);
 
     if (ok) rec.value = transition_penalty(sys.srv_cur_acc[s], sys.srv_cur_replicas[s], sys.srv_cur_cost[s], rec.acc,
                                            rec.numReplicas, rec.cost);
@@ -585,6 +615,135 @@ __global__ void k_pair_bucket_scatter(const long long* __restrict__ nIn, int nPa
     int b = n <= 0 ? 0 : (64 - __clzll(n));
     int pos = atomicAdd(&cursor[b], 1);
     order[pos] = t;
+}
+
+// ---------------------------------------------------------------------------------------
+// Pair sizing over a list of batch sizes (wva_analyze_pairs_batches)
+//   k_pairs_plane          one block per (server, accelerator) pair of a slice, every listed batch size b: the record
+//                          CreateAllocation returns under ServerSpec.MaxBatchSize = b, into column j of the plane
+//   k_pairs_plane_literal  the (pair, j) items k_pairs_plane sent to the materialised path, one thread each
+//   k_pairs_plane_best     SolveUnlimited per server over its A * n_b records (solver.go:63-79)
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ wva_pair_rec to_pair_rec(const AllocRec& r, bool ok) {
+    wva_pair_rec o;
+    o.acc = r.acc; o.feasible = ok ? 1 : 0; o.pad[0] = o.pad[1] = o.pad[2] = 0;
+    o.num_replicas = r.numReplicas; o.batch_size = r.batchSize;
+    o.cost = r.cost; o.value = r.value; o.itl = r.itl; o.ttft = r.ttft; o.rho = r.rho; o.max_arrv_rate_per_replica = r.maxArrv;
+    return o;
+}
+
+// servRate[n] does not depend on N (SURVEY Appendix D.4), so the pair's {rate, refined reciprocal} table is built once, in
+// shared memory, up to the list's largest b, and serves every item.  The block keeps the index of its first non-positive
+// or non-finite entry: item b needs the materialised path only when that index lies below b (k_pairs_warp tests the N
+// entries of its own table).  The warps pull batch indices from a shared counter, largest b first, and each sizes one
+// (pair, b) item with k_pairs_warp's body.  counters: [0] chain steps, [1..3] k_pairs_warp's round counters, [4] items
+// that reach the queue analyzer.
+__global__ void __launch_bounds__(WVA_PAIRS_WARP_THREADS)
+k_pairs_plane(DevSystem sys, int s0, const int* __restrict__ batch, int nB, wva_pair_rec* __restrict__ plane,
+              unsigned long long* slow_list, int* slow_count, unsigned long long* counters) {
+    extern __shared__ __align__(16) unsigned char plane_smem[];
+    __shared__ int nextItem, firstBad;
+    double2* tab = reinterpret_cast<double2*>(plane_smem);
+    const int pid = blockIdx.x;                       // pair relative to the slice: (s - s0) * A + a
+    const int s = s0 + pid / sys.A, a = pid % sys.A;
+    const int lane = threadIdx.x & 31;
+    // the pair reaches the queue analyzer (at every b alike) and so needs the table
+    const bool reach = is_candidate_accel(sys, s, a) && pair_lookups_ok(sys, s, a) && sys.srv_arrival_rpm[s] != 0.0f &&
+                       sys.srv_out_tokens[s] != 0;
+    if (threadIdx.x == 0) { nextItem = 0; firstBad = 0x7fffffff; }
+    __syncthreads();
+    if (reach) {
+        const size_t pi = (size_t)sys.srv_model[s] * sys.A + a;
+        ServiceParms sp; sp.alpha = sys.perf_alpha[pi]; sp.beta = sys.perf_beta[pi];
+        sp.gamma = sys.perf_gamma[pi]; sp.delta = sys.perf_delta[pi];
+        ServFormula sv;
+        sv.init(sp, sys.srv_in_tokens[s], sys.srv_out_tokens[s]);
+        const int bMax = batch[nB - 1];
+        for (int i = threadIdx.x; i < bMax; i += blockDim.x) {       // BuildModel (queueanalyzer.go:99-131)
+            const float r = sv.rate(i + 1);
+            if (!(r > 0.0f) || !(r < CUDART_INF_F)) atomicMin(&firstBad, i);
+            const double d = (double)r;
+            tab[i] = make_double2(d, rcp_refined(d));
+        }
+    }
+    __syncthreads();
+    const int fb = firstBad;
+    unsigned long long steps = 0;
+    int activeRounds = 0, totalRounds = 0, pendEvals = 0;
+    long long solveCycles = 0;
+    for (;;) {
+        int k = 0;
+        if (lane == 0) k = atomicAdd(&nextItem, 1);
+        k = __shfl_sync(0xffffffffu, k, 0);
+        if (k >= nB) break;
+        const int j = nB - 1 - k;
+        AllocRec rec = empty_alloc();
+        bool ok = false, toSlow = false;
+        auto table = [&](WarpPair& wp, long long N) -> double2* { wp.pstore = nullptr; return N <= fb ? tab : nullptr; };
+        size_pair_warp(sys, s, a, batch[j], table, lane, counters, rec, ok, toSlow, steps, activeRounds, totalRounds, pendEvals,
+                       solveCycles);
+        if (ok) rec.value = transition_penalty(sys.srv_cur_acc[s], sys.srv_cur_replicas[s], sys.srv_cur_cost[s], rec.acc,
+                                               rec.numReplicas, rec.cost);
+        if (lane == 0) {
+            const unsigned long long item = (unsigned long long)pid * nB + j;
+            if (toSlow) { ok = false; slow_list[atomicAdd(slow_count, 1)] = item; }
+            if (!ok) rec = empty_alloc();
+            plane[item] = to_pair_rec(rec, ok);
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) steps += __shfl_down_sync(0xffffffffu, steps, o);
+    if (lane == 0 && steps) atomicAdd(counters, steps);
+    if (threadIdx.x == 0 && reach) atomicAdd(counters + 4, (unsigned long long)nB);
+}
+
+// item = pair * nB + j of the slice; p[] materialised in HBM at scratch + scratch_off[t] (11 b + 1 doubles)
+__global__ void __launch_bounds__(64)
+k_pairs_plane_literal(DevSystem sys, int s0, const int* __restrict__ batch, int nB, const unsigned long long* __restrict__ list,
+                      int nList, double* scratch, const long long* __restrict__ scratch_off, wva_pair_rec* __restrict__ plane,
+                      unsigned long long* step_counter) {
+    int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nList) return;
+    const unsigned long long item = list[t];
+    const int pid = (int)(item / (unsigned long long)nB), j = (int)(item % (unsigned long long)nB);
+    const int s = s0 + pid / sys.A, a = pid % sys.A;
+    AllocRec rec = empty_alloc();
+    int fault = 0;
+    unsigned long long steps = 0;
+    bool ok = calculate_pair_n(sys, s, a, batch[j], scratch + scratch_off[t], rec, fault, steps);
+    if (!ok) rec = empty_alloc();
+    plane[item] = to_pair_rec(rec, ok);
+    atomicAdd(step_counter, steps);
+}
+
+// One warp per server.  Each lane scans its records in increasing scan position (a, then j) with the reference's strict
+// `<` from MaxFloat32, so it keeps the first of equal values; the warp then takes the least value, the lower scan
+// position on a tie.  Values compare as floats: -0 == +0, and NaN never passes `<`.
+__global__ void k_pairs_plane_best(const wva_pair_rec* __restrict__ plane, int ns, int perServer, wva_pair_rec* __restrict__ best) {
+    const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (w >= ns) return;
+    const wva_pair_rec* row = plane + (size_t)w * perServer;
+    float bv = __int_as_float(0x7f7fffff);     // math.MaxFloat32
+    int bi = -1;
+    for (int i = lane; i < perServer; i += 32) {
+        const float v = row[i].value;
+        if (row[i].feasible && v < bv) { bv = v; bi = i; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_down_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_down_sync(0xffffffffu, bi, o);
+        if (oi >= 0 && (bi < 0 || ov < bv || (ov == bv && oi < bi))) { bv = ov; bi = oi; }
+    }
+    if (lane == 0) {
+        wva_pair_rec r;
+        if (bi >= 0) r = row[bi];
+        else {
+            r.acc = WVA_ACC_NONE; r.feasible = 0; r.pad[0] = r.pad[1] = r.pad[2] = 0;
+            r.num_replicas = 0; r.batch_size = 0;
+            r.cost = r.value = r.itl = r.ttft = r.rho = r.max_arrv_rate_per_replica = 0.0f;
+        }
+        best[w] = r;
+    }
 }
 
 // ---------------------------------------------------------------------------------------

@@ -25,6 +25,8 @@ _Static_assert(offsetof(wva_system_soa, srv_cur_cost) == 16 + 26 * sizeof(void*)
 _Static_assert(sizeof(wva_alloc_soa) == 9 * sizeof(void*), "9 array pointers");
 _Static_assert(offsetof(wva_alloc_soa, max_arrv_rate_per_replica) == 8 * sizeof(void*), "last pointer");
 _Static_assert(WVA_COMM_ID_BYTES == 128, "ncclUniqueId");
+_Static_assert(sizeof(wva_pair_rec) == 48, "wva_pair_rec");
+_Static_assert(offsetof(wva_pair_rec, num_replicas) == 8 && offsetof(wva_pair_rec, max_arrv_rate_per_replica) == 44, "wva_pair_rec");
 
 enum { S = 6, A = 3, M = 6, T = 2 };
 
@@ -83,7 +85,24 @@ int main(void) {
     CHECK(nfe > 0);
     int64_t cnt[T]; float cst[T];
     CHECK(wva_allocate_by_type(ctx, cnt, cst) == WVA_OK);
-    printf("cabi_test: ok (%d feasible pairs, type counts %lld %lld)\n", nfe, (long long)cnt[0], (long long)cnt[1]);
+    /* pair sizing over a batch-size list: column j equals wva_pairs_fetch after an upload with that override */
+    const int32_t batch[3] = {8, 24, 40};
+    wva_pair_rec plane[S * A * 3], best[S];
+    CHECK(wva_analyze_pairs_batches(ctx, 3, batch, plane, best) == WVA_OK);
+    for (int s = 0; s < S; ++s) smb[s] = batch[1];
+    CHECK(wva_system_upload(ctx, &h) == WVA_OK);
+    CHECK(wva_analyze_pairs(ctx, NULL, NULL) == WVA_OK);
+    CHECK(wva_pairs_fetch(ctx, &o2, fe2) == WVA_OK);
+    int nb = 0;
+    for (int i = 0; i < S * A; ++i) {
+        const wva_pair_rec* r = &plane[i * 3 + 1];
+        CHECK(r->acc == acc2[i] && r->feasible == fe2[i] && r->num_replicas == rep2[i] && r->batch_size == bat2[i]);
+        CHECK(!memcmp(&r->cost, &f2[0][i], 4) && !memcmp(&r->value, &f2[1][i], 4) && !memcmp(&r->itl, &f2[2][i], 4));
+        CHECK(!memcmp(&r->ttft, &f2[3][i], 4) && !memcmp(&r->rho, &f2[4][i], 4) && !memcmp(&r->max_arrv_rate_per_replica, &f2[5][i], 4));
+        nb += r->feasible;
+    }
+    CHECK(nb > 0);
+    printf("cabi_test: ok (%d feasible pairs, type counts %lld %lld, %d at batch size 24)\n", nfe, (long long)cnt[0], (long long)cnt[1], nb);
     wva_ctx_destroy(ctx);
     return 0;
 }
