@@ -187,15 +187,19 @@ int wva_system_upload(wva_ctx* ctx, const wva_system_soa* host);
 /* Incremental updates of the RESIDENT image (System.AddServerFromSpec / RemoveServer / SetCountFromSpec /
  * Model.AddPerfDataFromSpec, pkg/core/system.go:99-171, model.go:45-54): only the touched rows cross PCIe.
  * wva_system_upload lays the arrays out with spare rows (1/16 more, at least 64); an update that would
- * outgrow them fails with WVA_ECAPACITY and the caller uploads the whole image again.  Every update
- * invalidates previous analysis results and resets the shard to "everything".
+ * outgrow them fails with WVA_ECAPACITY and the caller uploads the whole image again.  Every update that
+ * changes rows invalidates previous analysis results (pair records, decisions, sweep results) and resets the
+ * shard to "everything".  An update that fails changes nothing: image, dimensions, shard, wva_upload_bytes and
+ * results stay as they were.  A zero-row update (count == 0, after the same argument checks) is a no-op that
+ * keeps results and shard; wva_upload_bytes then reports 0.
  *   wva_system_update_servers: overwrite server rows [first, first+count) from rows->srv_* (arrays of
  *       `count` entries; rows->n_servers == count); first + count may extend the image (first <= S);
  *   wva_system_update_models:  overwrite the perf rows of models [first, first+count) from rows->perf_*
  *       (count * A entries; rows->n_models == count); may extend M the same way;
  *   wva_system_remove_server:  the last server's row moves into `index` (device-side), S shrinks by one --
  *       the host keeps its name -> index map in step;
- *   wva_system_set_capacity:   the T capacity counters.
+ *   wva_system_set_capacity:   the T capacity counters; it invalidates only the decisions of wva_solve (pair
+ *       records, sweep results and the shard stay).
  * wva_upload_bytes: bytes the last upload / update call moved host -> device. */
 #define WVA_ECAPACITY  -6   /* the resident image has no spare row left: upload again */
 int wva_system_update_servers(wva_ctx* ctx, int32_t first, int32_t count, const wva_system_soa* rows);
@@ -326,9 +330,11 @@ int wva_set_certified_tails(wva_ctx* ctx, int32_t on);
  * throughput).  Results do not depend on it.  Default 2^22 (the warp kernel's lanes stay converged, those of the
  * thread-per-pair kernel diverge); 0 = always thread-per-pair. */
 int wva_pairs_set_warp_max(wva_ctx* ctx, int32_t max_pairs);
-/* Tuning (warp-per-pair kernel): keep the chain values of pass 1 in HBM and read them back in pass 2
- * instead of re-running the recurrence.  Same results; off by default (the loads expose L2 latency that
- * the recomputation does not have). */
+/* Tuning (warp-per-pair kernel): bit 0 keeps the chain values of pass 1 in HBM and reads them back in pass 2
+ * instead of re-running the recurrence (off by default: the loads expose L2 latency that the recomputation does not
+ * have); bit 1 keeps every pair's rate table in HBM instead of the warp's shared-memory slice; bit 2 records
+ * wva_pair_debug's counters.  Same results in every mode.  May be called between two calls on the same image: a change
+ * of bit 1 makes the next wva_analyze_pairs plan the HBM tables again; no result is invalidated. */
 int wva_pairs_set_pstore(wva_ctx* ctx, int32_t on);
 /* Chain-state updates executed by the last wva_analyze_pairs (instrumentation). */
 int wva_pair_steps(wva_ctx* ctx, uint64_t* steps);

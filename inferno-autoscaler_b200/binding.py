@@ -214,6 +214,8 @@ class Context:
         """overwrite / append server rows [first, first+rows.S) from `rows` (its server arrays); self.image follows"""
         s = rows.c_struct()
         self._ck(lib().wva_system_update_servers(self._h, int(first), rows.S, C.byref(s)))
+        if rows.S == 0:
+            return              # a zero-row update changes nothing, the shard included
         img = self.image
         newS = max(img.S, first + rows.S)
         for name, dt in abi.SRV_FIELDS:
@@ -228,6 +230,8 @@ class Context:
     def update_models(self, first, rows: SystemImage):
         s = rows.c_struct()
         self._ck(lib().wva_system_update_models(self._h, int(first), rows.M, C.byref(s)))
+        if rows.M == 0:
+            return
         img = self.image
         newM = max(img.M, first + rows.M)
         for name, dt in abi.PERF_FIELDS:

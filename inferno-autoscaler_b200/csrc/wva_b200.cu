@@ -728,7 +728,10 @@ int wva_set_certified_tails(wva_ctx* ctx, int32_t on) {
 int wva_pairs_set_pstore(wva_ctx* ctx, int32_t on) {
     if (!ctx) return WVA_EINVAL;
     ctx->pairs_pstore = (on & 1) ? 1 : 0;
-    ctx->pairs_smem = (on & 2) ? 0 : 1;        // bit 1: keep the tables in HBM instead of shared memory (tuning/debug)
+    const int smem = (on & 2) ? 0 : 1;         // bit 1: keep the tables in HBM instead of shared memory (tuning/debug)
+    // the table plan gives pairs whose table sits in shared memory no HBM room: it is made again for the new placement
+    if (smem != ctx->pairs_smem) ctx->plan_valid = false;
+    ctx->pairs_smem = smem;
     ctx->pairs_debug = (on & 4) ? 1 : 0;       // bit 2: record per-pair cycles / rounds (wva_pair_debug)
     return WVA_OK;
 }
