@@ -322,6 +322,32 @@ func (c *Context) PairsAtBatchSizes(batches []int32, wantPlane bool) (plane, bes
 		"wva_analyze_pairs_batches")
 }
 
+// PairsAtArrivalRates sizes every pair of the shard under each of nLoads arrival-rate scenarios: rpm[(srv-first)*nLoads+j]
+// is the server's ServerLoadSpec.ArrivalRate (req/min) in scenario j.  plane[((srv-first)*nLoads+j)*A+a] is
+// CreateAllocation's record of pair (srv, a) at that rate (nil unless wantPlane), best[(srv-first)*nLoads+j] is
+// SolveUnlimited over those A records.  QueueAnalyzer.Size runs once per pair.  The slices are sized from the library's
+// own shard and dimensions.  The resident image, pair records, decisions and sweep results are left as they were.
+func (c *Context) PairsAtArrivalRates(rpm []float32, nLoads int, wantPlane bool) (plane, best []PairRec, err error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var S, A, M, T, first, count C.int32_t
+	if err = c.err(C.wva_system_dims(c.ctx, &S, &A, &M, &T), "wva_system_dims"); err != nil {
+		return nil, nil, err
+	}
+	if err = c.err(C.wva_shard_info(c.ctx, &first, &count), "wva_shard_info"); err != nil {
+		return nil, nil, err
+	}
+	if nLoads < 1 || len(rpm) != int(count)*nLoads {
+		return nil, nil, fmt.Errorf("PairsAtArrivalRates: rpm needs count*nLoads = %d*%d rates, got %d", int(count), nLoads, len(rpm))
+	}
+	best = make([]PairRec, int(count)*nLoads)
+	if wantPlane {
+		plane = make([]PairRec, int(count)*nLoads*int(A))
+	}
+	return plane, best, c.err(C.wva_analyze_pairs_loads(c.ctx, C.int32_t(nLoads), f32p(rpm), pairRecs(plane), pairRecs(best)),
+		"wva_analyze_pairs_loads")
+}
+
 // QueueConfig is wva_queue_config; Metrics is wva_metrics (analyzer.AnalysisMetrics).
 type QueueConfig struct {
 	MaxBatchSize, MaxQueueSize int32
@@ -463,6 +489,26 @@ func (g *Group) PairsAtBatchSizes(batches []int32, wantPlane bool) (plane, best 
 	}
 	return plane, best, g.err(C.wva_group_analyze_pairs_batches(g.g, C.int32_t(len(batches)), i32p(batches), pairRecs(plane), pairRecs(best)),
 		"wva_group_analyze_pairs_batches")
+}
+
+// PairsAtArrivalRates: Context.PairsAtArrivalRates over every device's servers, assembled: rpm holds S*nLoads rates
+// (sized from device 0's image).
+func (g *Group) PairsAtArrivalRates(rpm []float32, nLoads int, wantPlane bool) (plane, best []PairRec, err error) {
+	g.mu.Lock()
+	defer g.mu.Unlock()
+	var S, A, M, T C.int32_t
+	if rc := C.wva_system_dims(C.wva_group_ctx(g.g, 0), &S, &A, &M, &T); rc != C.WVA_OK {
+		return nil, nil, fmt.Errorf("wva_system_dims: %d", int(rc))
+	}
+	if nLoads < 1 || len(rpm) != int(S)*nLoads {
+		return nil, nil, fmt.Errorf("PairsAtArrivalRates: rpm needs S*nLoads = %d*%d rates, got %d", int(S), nLoads, len(rpm))
+	}
+	best = make([]PairRec, int(S)*nLoads)
+	if wantPlane {
+		plane = make([]PairRec, int(S)*nLoads*int(A))
+	}
+	return plane, best, g.err(C.wva_group_analyze_pairs_loads(g.g, C.int32_t(nLoads), f32p(rpm), pairRecs(plane), pairRecs(best)),
+		"wva_group_analyze_pairs_loads")
 }
 
 // AllocateByType: global per-type totals (NCCL all-gather of the partials inside the library).

@@ -376,6 +376,33 @@ int wva_analyze_pairs_batches(wva_ctx* ctx, int32_t n_b, const int32_t* batch, w
  * path, chain steps executed, items sized (those that reached the queue analyzer)}. */
 int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]);
 
+/* Pair sizing over a matrix of arrival-rate scenarios.  arrival_rpm[(s - s0) * n_l + j] is server s's
+ * ServerLoadSpec.ArrivalRate (requests per minute) in scenario j, for the servers of the shard; 1 <= n_l <= 8192.
+ * Record (s, j, a) is the record wva_pairs_fetch gives for pair (s, a) after uploading the same image with
+ * srv_arrival_rpm[s] = arrival_rpm[(s - s0) * n_l + j]: candidate filter, the nil lookups (a negative rate gives nil),
+ * the zero-load record for +0 and -0, CreateAllocation, value = TransitionPenalty against the uploaded current
+ * allocation, the empty record with feasible = 0 where CreateAllocation returns nil.  A positive rate whose totalRate
+ * is 0 (rpm / 60 below about 4.2e-44 on a server without a TPS target) on a server with MinNumReplicas <= 0 also gives
+ * the empty record: numReplicas is 0 there and the reference's Analyze(0 / 0) never returns.
+ *   plane [servers of the shard * n_l * A], index ((s - s0) * n_l + j) * A + a, or NULL (not copied to the host): the A
+ *         records of one (server, scenario) are contiguous;
+ *   best  [servers of the shard * n_l], index (s - s0) * n_l + j, or NULL: SolveUnlimited (pkg/solver/solver.go:63-79)
+ *         over those A records -- wva_solve(unlimited)'s chosen record on the same image with feasible = 1, or the empty
+ *         record (acc = -1, feasible = 0) where it chooses none.
+ * QueueAnalyzer.Size does not read the load, so it runs once per pair whatever n_l is.  The records are staged in HBM in
+ * slices of at most 2^28 bytes of servers (one server at least): each slice's rows of arrival_rpm are copied in and its
+ * records copied out before the next starts.  Items that need the materialised-p[] path run in chunks that fit half
+ * the free device memory; WVA_ECUDA only when one item alone does not fit (where wva_analyze_pairs fails too).  Nothing that other calls read changes: pair records, decisions, totals,
+ * sweep results and the resident image (srv_arrival_rpm included), and whether they are valid, stay as they were.
+ * WVA_EINVAL for n_l out of range, arrival_rpm == NULL while the shard has servers, or a NaN rate (the reference's
+ * Analyze does not return on it); WVA_ESTATE before any upload.  Both change nothing. */
+#define WVA_PAIRS_MAX_LOADS 8192
+int wva_analyze_pairs_loads(wva_ctx* ctx, int32_t n_l, const float* arrival_rpm, wva_pair_rec* plane, wva_pair_rec* best);
+/* Counters of the last wva_analyze_pairs_loads: {server slices, pairs that reach QueueAnalyzer.Size (counted once
+ * per pair however many scenarios it serves), (pair, scenario) items that reached the final Analyze, items sent to the materialised-p[]
+ * path, chain steps executed}. */
+int wva_pairs_loads_counters(const wva_ctx* ctx, uint64_t out[5]);
+
 /* ---- Optimize ------------------------------------------------------------ */
 
 /* Replaces solver.Solver.Solve (pkg/solver/solver.go:32-60): SolveUnlimited (:63-79) or
@@ -470,6 +497,8 @@ int wva_group_analyze(wva_group* g, int32_t r_max, int32_t b_max, int32_t want_c
 int wva_group_pairs_fetch(wva_group* g, wva_alloc_soa* out, uint8_t* feasible);
 int wva_group_grid_fetch(wva_group* g, wva_grid_best* best /* [S] */);
 int wva_group_grid_best_blocking(wva_group* g, float* p_block /* [S] */);   /* wva_grid_best_blocking, assembled */
+int wva_group_analyze_pairs_loads(wva_group* g, int32_t n_l, const float* arrival_rpm /* [S*n_l] */,
+                                  wva_pair_rec* plane /* [S*n_l*A] */, wva_pair_rec* best /* [S*n_l] */);   /* assembled */
 int wva_group_analyze_pairs_batches(wva_group* g, int32_t n_b, const int32_t* batch,
                                     wva_pair_rec* plane /* [S*A*n_b] */, wva_pair_rec* best /* [S] */);   /* assembled */
 int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen);

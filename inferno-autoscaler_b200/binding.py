@@ -32,6 +32,7 @@ EXPORTS = [
     "wva_grid_blocking", "wva_grid_blocking_size", "wva_grid_blocking_device", "wva_grid_best_blocking", "wva_grid_blocking_counts", "wva_grid_blocking_exact_fetch",
     "wva_group_grid_best_blocking",
     "wva_analyze_pairs_batches", "wva_pairs_batches_counters", "wva_group_analyze_pairs_batches", "wva_shard_info",
+    "wva_analyze_pairs_loads", "wva_pairs_loads_counters", "wva_group_analyze_pairs_loads",
 ]
 
 
@@ -136,6 +137,9 @@ def lib():
         L.wva_pairs_batches_counters.argtypes = [vp, C.POINTER(u64)]
         L.wva_group_analyze_pairs_batches.argtypes = [vp, i32, abi.i32p, vp, vp]
         L.wva_shard_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
+        L.wva_analyze_pairs_loads.argtypes = [vp, i32, abi.f32p, vp, vp]
+        L.wva_pairs_loads_counters.argtypes = [vp, C.POINTER(u64)]
+        L.wva_group_analyze_pairs_loads.argtypes = [vp, i32, abi.f32p, vp, vp]
         if L.wva_abi_version() != abi.ABI_VERSION:
             raise ImportError("libwva_b200.so ABI version mismatch")
         _lib = L
@@ -312,6 +316,28 @@ class Context:
         v = (C.c_uint64 * 4)()
         self._ck(lib().wva_pairs_batches_counters(self._h, v))
         return dict(slices=v[0], materialised=v[1], steps=v[2], sized=v[3])
+
+    def analyze_pairs_loads(self, rpm, plane=True):
+        """Pair sizing under each arrival-rate scenario: rpm [count, n_l] holds the shard's servers'
+        ServerLoadSpec.ArrivalRate (req/min) per scenario.  Returns (plane, best), numpy arrays of abi.PAIR_REC_DTYPE:
+        plane [count, n_l, A] with plane[s - first, j, a] the record of pair (s, a) at rate rpm[s - first, j], or None
+        when plane=False (it then stays off PCIe); best [count, n_l] is SolveUnlimited over each (server, scenario)'s A
+        records.  The resident image and results are left as they were."""
+        r = np.ascontiguousarray(rpm, dtype=np.float32)
+        if r.ndim != 2 or r.shape[0] != self.count:
+            raise ValueError("rpm must be shaped [count, n_l]")
+        n_l = r.shape[1]
+        best = np.zeros((self.count, n_l), dtype=abi.PAIR_REC_DTYPE)
+        pl = np.zeros((self.count, n_l, self.image.A), dtype=abi.PAIR_REC_DTYPE) if plane else None
+        self._ck(lib().wva_analyze_pairs_loads(self._h, n_l, abi.ptr(r, C.c_float), pl.ctypes.data if plane else None,
+                                               best.ctypes.data))
+        return pl, best
+
+    def pairs_loads_counters(self):
+        """counters of the last analyze_pairs_loads"""
+        v = (C.c_uint64 * 5)()
+        self._ck(lib().wva_pairs_loads_counters(self._h, v))
+        return dict(slices=v[0], sized_pairs=v[1], analyzed=v[2], materialised=v[3], steps=v[4])
 
     def pair_counters(self):
         v = (C.c_uint64 * 4)()
@@ -607,6 +633,19 @@ class Group:
         pl = np.zeros((self.image.S * self.image.A, len(b)), dtype=abi.PAIR_REC_DTYPE) if plane else None
         self._ck(lib().wva_group_analyze_pairs_batches(self._h, len(b), abi.ptr(b, C.c_int32),
                                                        pl.ctypes.data if plane else None, best.ctypes.data))
+        return pl, best
+
+    def analyze_pairs_loads(self, rpm, plane=True):
+        """Context.analyze_pairs_loads over every device's servers, assembled: rpm [S, n_l] -> plane [S, n_l, A],
+        best [S, n_l]"""
+        r = np.ascontiguousarray(rpm, dtype=np.float32)
+        if r.ndim != 2 or r.shape[0] != self.image.S:
+            raise ValueError("rpm must be shaped [S, n_l]")
+        n_l = r.shape[1]
+        best = np.zeros((self.image.S, n_l), dtype=abi.PAIR_REC_DTYPE)
+        pl = np.zeros((self.image.S, n_l, self.image.A), dtype=abi.PAIR_REC_DTYPE) if plane else None
+        self._ck(lib().wva_group_analyze_pairs_loads(self._h, n_l, abi.ptr(r, C.c_float), pl.ctypes.data if plane else None,
+                                                     best.ctypes.data))
         return pl, best
 
     def solve(self, unlimited=True, delayed_best_effort=False, policy=abi.POLICY_NONE, download=True):

@@ -191,6 +191,9 @@ struct wva_ctx {
     // wva_analyze_pairs_batches: buffers of its own, so the resident pair results above stay as they are
     DevBuf pbBatch, pbSlow, pbScratch, pbScratchOff, pbPlane, pbBest, pbCount;
     uint64_t pb_counters[4] = {0, 0, 0, 0};
+    // wva_analyze_pairs_loads: likewise, with a table plan of its own
+    DevBuf plRpm, plSlow, plScratch, plScratchOff, plPlane, plBest, plCount, plTabOff, plTabs;
+    uint64_t pl_counters[5] = {0, 0, 0, 0, 0};
 
     // solution
     DevBuf chosenBuf; DevAllocs chosen{}; int* chosen_acc = nullptr; bool solved = false;
@@ -407,7 +410,9 @@ void wva_ctx_destroy(wva_ctx* ctx) {
                       &ctx->ioC, &ctx->ioD, &ctx->ioE, &ctx->ioF, &ctx->ioG, &ctx->commTotals, &ctx->commChunk, &ctx->commGather,
                       &ctx->blkPlane, &ctx->blkExact, &ctx->blkLit, &ctx->blkCount, &ctx->blkCounts, &ctx->blkScratch, &ctx->blkIo,
                       &ctx->pbBatch, &ctx->pbSlow, &ctx->pbScratch, &ctx->pbScratchOff,
-                      &ctx->pbPlane, &ctx->pbBest, &ctx->pbCount};
+                      &ctx->pbPlane, &ctx->pbBest, &ctx->pbCount,
+                      &ctx->plRpm, &ctx->plSlow, &ctx->plScratch, &ctx->plScratchOff, &ctx->plPlane, &ctx->plBest,
+                      &ctx->plCount, &ctx->plTabOff, &ctx->plTabs};
     for (DevBuf* b : bufs) b->release();
     ctx->staging.release();
     cudaEventDestroy(ctx->ev0);
@@ -446,29 +451,26 @@ int64_t wva_phase_time_usec(const wva_ctx* ctx, int phase) {
 }
 int64_t wva_solution_time_usec(const wva_ctx* ctx) { return wva_phase_time_usec(ctx, WVA_PHASE_SOLVE); }
 
-// N of CreateAllocation (allocation.go:77-87) per pair of servers [s0, s1), or an upper bound where the device
+// N of CreateAllocation (allocation.go:77-87) for pair (s, a) under a positive load, or an upper bound where the
+// device finds the pair unusable; 0 when the pair reaches the queue analyzer under no load (no output tokens)
+static long long host_pair_n(const wva_ctx* ctx, int s, int a) {
+    const int m = ctx->h_srv_model[(size_t)s];
+    const long long outTok = ctx->h_srv_out[(size_t)s];
+    if (outTok == 0) return 0;
+    if (ctx->h_srv_mb[(size_t)s] > 0) return ctx->h_srv_mb[(size_t)s];
+    if (m < 0) return 0;
+    const size_t pi = (size_t)m * ctx->A + a;
+    const long long prod = (long long)((unsigned long long)(long long)ctx->h_pmb[pi] * (unsigned long long)(long long)ctx->h_pat[pi]);
+    const long long n = (outTok == -1) ? (long long)(0ull - (unsigned long long)prod) : prod / outTok;
+    return n < 1 ? 1 : n;
+}
+// N of CreateAllocation per pair of servers [s0, s1) under the uploaded load, or an upper bound where the device
 // finds the pair unusable (it then needs no table at all): sizes the tables of the warp-per-pair kernel
 // without a device round trip
 static void host_plan_rows(wva_ctx* ctx, int s0, int s1) {
     const int A = ctx->A;
-    for (int s = s0; s < s1; ++s) {
-        const int m = ctx->h_srv_model[(size_t)s];
-        const long long outTok = ctx->h_srv_out[(size_t)s];
-        for (int a = 0; a < A; ++a) ctx->hostN[(size_t)s * A + a] = 0;
-        if (ctx->h_srv_arr[(size_t)s] == 0.0f || outTok == 0) continue;
-        for (int a = 0; a < A; ++a) {
-            long long n;
-            if (ctx->h_srv_mb[(size_t)s] > 0) n = ctx->h_srv_mb[(size_t)s];
-            else if (m < 0) n = 0;
-            else {
-                const size_t pi = (size_t)m * A + a;
-                const long long prod = (long long)((unsigned long long)(long long)ctx->h_pmb[pi] * (unsigned long long)(long long)ctx->h_pat[pi]);
-                n = (outTok == -1) ? (long long)(0ull - (unsigned long long)prod) : prod / outTok;
-                if (n < 1) n = 1;
-            }
-            ctx->hostN[(size_t)s * A + a] = n;
-        }
-    }
+    for (int s = s0; s < s1; ++s)
+        for (int a = 0; a < A; ++a) ctx->hostN[(size_t)s * A + a] = ctx->h_srv_arr[(size_t)s] == 0.0f ? 0 : host_pair_n(ctx, s, a);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -855,6 +857,138 @@ int wva_shard_info(const wva_ctx* ctx, int32_t* first, int32_t* count) {
 int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]) {
     if (!ctx || !out) return WVA_EINVAL;
     for (int k = 0; k < 4; ++k) out[k] = ctx->pb_counters[k];
+    return WVA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Pair sizing over a matrix of arrival-rate scenarios.  Per slice of servers: the slice's rows of rates go to the
+// device, k_pairs_loads sizes each pair once and writes its record under every scenario, k_pairs_loads_literal re-runs
+// the items it sent to the materialised path, k_pairs_plane_best picks each (server, scenario)'s record, and the slice
+// is copied out before the next one starts.  The rate tables are planned here from N under a positive load: the plan
+// of wva_analyze_pairs follows the uploaded rates and gives a zero-load server no table.  Buffers of its own: the
+// resident pair results and the resident image stay as they are.
+int wva_analyze_pairs_loads(wva_ctx* ctx, int32_t n_l, const float* arrival_rpm, wva_pair_rec* plane, wva_pair_rec* best) {
+    if (!ctx) return WVA_EINVAL;
+    if (n_l < 1 || n_l > WVA_PAIRS_MAX_LOADS) return fail(ctx, WVA_EINVAL, "scenario count: 1 <= n_l <= 8192 required");
+    if (!ctx->have_system) return fail(ctx, WVA_ESTATE, "no system uploaded");
+    const int A = ctx->A, ns = ctx->ns;
+    if (ns > 0 && !arrival_rpm) return fail(ctx, WVA_EINVAL, "arrival_rpm is NULL");
+    const size_t nRates = (size_t)ns * (size_t)n_l;
+    for (size_t i = 0; i < nRates; ++i)
+        if (arrival_rpm[i] != arrival_rpm[i]) return fail(ctx, WVA_EINVAL, "NaN arrival rate (the reference's Analyze does not return on it)");
+    const size_t perServer = (size_t)A * (size_t)n_l;
+    if (perServer > 0x7fffffffULL) return fail(ctx, WVA_EINVAL, "A * n_l exceeds 2^31-1");
+    CK(cudaSetDevice(ctx->device));
+    for (int k = 0; k < 5; ++k) ctx->pl_counters[k] = 0;
+    if (ns == 0) return WVA_OK;
+    const size_t recBytes = perServer * sizeof(wva_pair_rec);
+    const int slice = (int)std::max<size_t>(1, std::min<size_t>((size_t)ns, ((size_t)1 << 28) / recBytes));
+    const size_t maxItems = (size_t)slice * perServer;
+    CK(ctx->plRpm.ensure((size_t)slice * n_l * 4));
+    CK(ctx->plSlow.ensure(maxItems * 8));
+    CK(ctx->plPlane.ensure((size_t)slice * recBytes));
+    CK(ctx->plBest.ensure((size_t)slice * n_l * sizeof(wva_pair_rec)));
+    CK(ctx->plTabOff.ensure((size_t)slice * A * 8));
+    CK(ctx->plCount.ensure(64));
+    // [0, 4) slow-list length, [8, 56) k_pairs_loads's counters
+    char* cnt = ctx->plCount.as<char>();
+    int* slowCount = reinterpret_cast<int*>(cnt);
+    unsigned long long* counters = reinterpret_cast<unsigned long long*>(cnt + 8);
+    CK(cudaMemsetAsync(cnt, 0, 64, ctx->stream));
+    float* dRpm = ctx->plRpm.as<float>();
+    wva_pair_rec* dPlane = ctx->plPlane.as<wva_pair_rec>();
+    wva_pair_rec* dBest = ctx->plBest.as<wva_pair_rec>();
+    unsigned long long* dSlow = ctx->plSlow.as<unsigned long long>();
+    const int warpsPerBlock = WVA_PAIRS_WARP_THREADS / 32;
+    const long long budget = (2LL << 30) / 16;           // at most 2 GB of tables, as wva_analyze_pairs
+    std::vector<long long> nPair, offs;
+    std::vector<unsigned long long> items;
+    std::vector<long long> soffs;
+    uint64_t nSlices = 0, nSlow = 0;
+    for (int f = ctx->s0; f < ctx->s0 + ns; f += slice) {
+        const int nss = std::min(slice, ctx->s0 + ns - f);
+        const int nPairs = nss * A;
+        const size_t hs = (size_t)(f - ctx->s0);
+        // table plan: the warp's shared-memory slice up to 3072 entries, HBM above that under the budget, the
+        // materialised path beyond it or above 2^26 entries
+        nPair.resize((size_t)nPairs);
+        offs.resize((size_t)nPairs);
+        long long maxN = 0, total = 0;
+        for (int i = 0; i < nPairs; ++i) {
+            const long long N = host_pair_n(ctx, f + i / A, i % A);
+            nPair[(size_t)i] = N;
+            if (N > maxN && N <= (1LL << 26)) maxN = N;
+        }
+        const long long inSmem = ctx->pairs_smem ? (maxN < 3072 ? maxN : 3072) : 0;
+        for (int i = 0; i < nPairs; ++i) {
+            const long long N = nPair[(size_t)i];
+            if (N <= 0 || N <= inSmem) { offs[(size_t)i] = 0; continue; }
+            if (N > (1LL << 26) || total + N > budget) { offs[(size_t)i] = -1; continue; }
+            offs[(size_t)i] = total; total += N;
+        }
+        CK(ctx->plTabs.ensure((size_t)(total ? total : 1) * 16));
+        CK(cudaMemcpyAsync(ctx->plTabOff.p, offs.data(), (size_t)nPairs * 8, cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(dRpm, arrival_rpm + hs * n_l, (size_t)nss * n_l * 4, cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemsetAsync(slowCount, 0, 4, ctx->stream));
+        const int smemEntries = (int)inSmem;
+        const size_t smemBytes = (size_t)smemEntries * 16 * warpsPerBlock;
+        if (smemBytes > 48 * 1024) CK(cudaFuncSetAttribute(k_pairs_loads, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+        k_pairs_loads<<<(nPairs + warpsPerBlock - 1) / warpsPerBlock, WVA_PAIRS_WARP_THREADS, smemBytes, ctx->stream>>>(
+            ctx->dsys, f, nPairs, n_l, dRpm, ctx->plTabOff.as<long long>(), ctx->plTabs.as<double2>(), smemEntries, dPlane, dSlow,
+            slowCount, counters);
+        LAUNCH_CHECK();
+        int slow = 0;
+        CK(cudaMemcpyAsync(&slow, slowCount, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (slow > 0) {
+            // items whose chain hit an overflow-rescale branch, or whose pair has no usable table: p[] in HBM.  A pair
+            // can send all n_l of its items here, so they run in chunks whose scratch fits half the free memory: the call
+            // fails only when a single item does not fit, where wva_analyze_pairs fails too.
+            items.resize((size_t)slow);
+            soffs.resize((size_t)slow);
+            CK(cudaMemcpy(items.data(), dSlow, (size_t)slow * 8, cudaMemcpyDeviceToHost));
+            size_t freeB = 0, totB = 0;
+            CK(cudaMemGetInfo(&freeB, &totB));
+            const size_t capB = std::max(freeB / 2, ctx->plScratch.cap);
+            for (int i0 = 0; i0 < slow;) {
+                long long stotal = 0;
+                int i1 = i0;
+                for (; i1 < slow; ++i1) {
+                    const unsigned long long it = items[(size_t)i1];
+                    const long long N = nPair[(size_t)((it / (unsigned long long)A) / (unsigned long long)n_l * A + it % (unsigned long long)A)];
+                    if (N > (1LL << 32)) return fail(ctx, WVA_EINVAL, "pair needs the materialised path with an unreasonably large batch size");
+                    if (i1 > i0 && (size_t)(stotal + 11 * N + 1) * 8 > capB) break;
+                    soffs[(size_t)(i1 - i0)] = stotal; stotal += 11 * N + 1;
+                }
+                if ((size_t)stotal * 8 > capB) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
+                const int n = i1 - i0;
+                CK(ctx->plScratch.ensure((size_t)stotal * 8));
+                CK(ctx->plScratchOff.ensure((size_t)n * 8));
+                CK(cudaMemcpyAsync(ctx->plScratchOff.p, soffs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+                k_pairs_loads_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, n_l, dRpm, dSlow + i0, n, ctx->plScratch.as<double>(),
+                                                                            ctx->plScratchOff.as<long long>(), dPlane, counters);
+                LAUNCH_CHECK();
+                CK(cudaStreamSynchronize(ctx->stream));      // the next chunk reuses the scratch and its offsets
+                i0 = i1;
+            }
+            nSlow += (uint64_t)slow;
+        }
+        k_pairs_plane_best<<<(nss * n_l + 3) / 4, 128, 0, ctx->stream>>>(dPlane, nss * n_l, A, dBest);
+        LAUNCH_CHECK();
+        if (plane) CK(cudaMemcpyAsync(plane + hs * perServer, dPlane, (size_t)nss * recBytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (best) CK(cudaMemcpyAsync(best + hs * n_l, dBest, (size_t)nss * n_l * sizeof(wva_pair_rec), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));       // also releases offs, soffs and the slice's buffers for the next slice
+        ++nSlices;
+    }
+    unsigned long long dev[6];
+    CK(cudaMemcpy(dev, counters, sizeof dev, cudaMemcpyDeviceToHost));
+    ctx->pl_counters[0] = nSlices; ctx->pl_counters[1] = dev[4]; ctx->pl_counters[2] = dev[5]; ctx->pl_counters[3] = nSlow;
+    ctx->pl_counters[4] = dev[0];
+    return WVA_OK;
+}
+int wva_pairs_loads_counters(const wva_ctx* ctx, uint64_t out[5]) {
+    if (!ctx || !out) return WVA_EINVAL;
+    for (int k = 0; k < 5; ++k) out[k] = ctx->pl_counters[k];
     return WVA_OK;
 }
 
@@ -2091,6 +2225,23 @@ int wva_group_grid_fetch(wva_group* g, wva_grid_best* best) {
 int wva_group_grid_best_blocking(wva_group* g, float* p_block) {
     if (!g || !p_block) return WVA_EINVAL;
     return g->each([&](int, wva_ctx* c) { return wva_grid_best_blocking(c, p_block + c->s0); });
+}
+
+int wva_group_analyze_pairs_loads(wva_group* g, int32_t n_l, const float* arrival_rpm, wva_pair_rec* plane, wva_pair_rec* best) {
+    if (!g) return WVA_EINVAL;
+    const bool okN = n_l >= 1 && n_l <= WVA_PAIRS_MAX_LOADS;       // otherwise every device fails with WVA_EINVAL
+    // a NaN anywhere fails the whole call before any device writes its rows
+    if (okN && arrival_rpm) {
+        size_t rows = 0;
+        for (wva_ctx* c : g->ctxs) if (c->have_system) rows = std::max(rows, (size_t)(c->s0 + c->ns));
+        for (size_t i = 0; i < rows * (size_t)n_l; ++i)
+            if (arrival_rpm[i] != arrival_rpm[i]) { g->err = "NaN arrival rate (the reference's Analyze does not return on it)"; return WVA_EINVAL; }
+    }
+    return g->each([&](int, wva_ctx* c) {
+        const size_t r0 = okN ? (size_t)c->s0 * (size_t)n_l : 0;     // the device's first (server, scenario) row
+        return wva_analyze_pairs_loads(c, n_l, arrival_rpm ? arrival_rpm + r0 : nullptr,
+                                       (plane && okN) ? plane + r0 * (size_t)c->A : nullptr, (best && okN) ? best + r0 : nullptr);
+    });
 }
 
 int wva_group_analyze_pairs_batches(wva_group* g, int32_t n_b, const int32_t* batch, wva_pair_rec* plane, wva_pair_rec* best) {

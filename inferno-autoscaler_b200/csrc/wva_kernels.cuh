@@ -317,11 +317,17 @@ __device__ __forceinline__ SolveStats shfl_stats(const SolveStats& s, int src) {
 // CreateAllocation by the warp (without the transition penalty).  table(wp, N) hands out the pair's {rate, reciprocal}
 // table of N entries, ready for use, or nullptr when the item must go to the materialised path.  Called by the 32 lanes
 // of a warp together.
-template <class Table>
+// With an AtLambda hook (k_pairs_loads), QueueAnalyzer.Size stops at the rate its bisections settle on: once
+// requestRate = lambda* * 1000 has passed Size's range test, atLambda(wp, st, lastX, requestRate, N) is called with the
+// warp's pair state (st / lastX: this lane's most recent evaluation and its lambda, lastX < 0 for none) and nothing
+// after it runs; rec and ok are left as they were.  If Size fails the hook is not called; toSlow says whether that was
+// the materialised path.  Without a hook (NoLambdaHook) the body is k_pairs_warp's as it always was.
+struct NoLambdaHook { static constexpr bool on = false; };
+template <class Table, class AtLambda = NoLambdaHook>
 __device__ __forceinline__ void size_pair_warp(const DevSystem& sys, int s, int a, long long over, Table table, int lane,
                                                unsigned long long* step_counter, AllocRec& rec, bool& ok, bool& toSlow,
                                                unsigned long long& steps, int& activeRounds, int& totalRounds, int& pendEvals,
-                                               long long& solveCycles) {
+                                               long long& solveCycles, AtLambda atLambda = AtLambda()) {
     // every lane runs the scalar part redundantly (uniform control flow)
     do {
         if (!is_candidate_accel(sys, s, a) || !pair_lookups_ok(sys, s, a)) break;
@@ -477,6 +483,7 @@ __device__ __forceinline__ void size_pair_warp(const DevSystem& sys, int s, int 
         const float requestRate = lambda * 1000.0f;
         // ---- Analyze(requestRate) (:237-241) and Analyze(totalRate/replicas) (allocation.go:148) ----
         if (requestRate <= 0.0f || requestRate > wp.rateMax) break;        // :135-143 -> Size fails -> nil
+        if constexpr (AtLambda::on) { atLambda(wp, st, lastX, requestRate, N); break; }
         const float x1 = requestRate / 1000.0f;
         float totalRate;
         if (tTPS == 0.0f) totalRate = arrival / 60.0f;
@@ -744,6 +751,210 @@ __global__ void k_pairs_plane_best(const wva_pair_rec* __restrict__ plane, int n
         }
         best[w] = r;
     }
+}
+
+// ---------------------------------------------------------------------------------------
+// Pair sizing over a matrix of arrival-rate scenarios (wva_analyze_pairs_loads)
+//   k_pairs_loads          one warp per (server, accelerator) pair of a slice: QueueAnalyzer.Size once, then every
+//                          scenario j's record CreateAllocation returns under ServerLoadSpec.ArrivalRate = rpm[j]
+//   k_pairs_loads_literal  the (pair, j) items k_pairs_loads sent to the materialised path, one thread each
+// Records go to plane[((s - s0) * nL + j) * A + a]: the A records of one (server, scenario) are contiguous, so
+// k_pairs_plane_best picks each (server, scenario)'s record over rows of A.
+// ---------------------------------------------------------------------------------------
+
+// The image as seen from server s alone: every server array starts at s, so server s is index 0, and its
+// ServerLoadSpec.ArrivalRate is *rate.  Lets the pair code of wva_analyze_pairs run one server at a scenario's rate.
+__device__ __forceinline__ DevSystem server_view(const DevSystem& sys, int s, const float* rate) {
+    DevSystem v = sys;
+    v.srv_model += s; v.srv_arrival_rpm = rate; v.srv_in_tokens += s; v.srv_out_tokens += s;
+    v.srv_slo_ttft += s; v.srv_slo_itl += s; v.srv_slo_tps += s; v.srv_target_valid += s;
+    v.srv_priority += s; v.srv_min_replicas += s; v.srv_max_batch += s; v.srv_keep_acc += s;
+    v.srv_cur_acc += s; v.srv_cur_replicas += s; v.srv_cur_cost += s;
+    return v;
+}
+
+// size_pair_warp's hook around a callable
+template <class F>
+struct LambdaHook {
+    static constexpr bool on = true;
+    F f;
+    __device__ __forceinline__ void operator()(const WarpPair& wp, const SolveStats& st, float lastX, float requestRate,
+                                               long long N) { f(wp, st, lastX, requestRate, N); }
+};
+
+// N, Size and rateStar read the perf row, the SLO targets and the token counts, never the load (allocation.go:77-131):
+// the warp sizes the pair once with size_pair_warp (stopped at lambda*, on the server seen at one of its sizing
+// scenarios), then its lanes take one scenario each.  A lane computes totalRate, numReplicas, cost and the per-replica
+// rate (:134-146); the final Analyze (:148) re-uses the Solve behind rateStar when the rate lands on the same lambda,
+// and otherwise runs on the lane, all lanes of a round side by side.  rpm: the slice's rows, nL per server, no NaN.
+// tabOff / tabs / smemEntriesPerWarp: the table plan for the slice's pairs, as k_pairs_warp's.
+// counters: [0] chain steps, [1..2] Size's round counters, [4] pairs that reach Size (once each), [5] items that reached
+// the final Analyze.
+__global__ void __launch_bounds__(WVA_PAIRS_WARP_THREADS)
+k_pairs_loads(DevSystem sys, int s0, int nPairs, int nL, const float* __restrict__ rpm, const long long* __restrict__ tabOff,
+              double2* tabs, int smemEntriesPerWarp, wva_pair_rec* __restrict__ plane, unsigned long long* slow_list,
+              int* slow_count, unsigned long long* counters) {
+    extern __shared__ __align__(16) unsigned char loads_smem[];
+    const int pid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;      // (s - s0) * A + a, warp-uniform
+    const int lane = threadIdx.x & 31;
+    if (pid >= nPairs) return;
+    const int A = sys.A, sl = pid / A, s = s0 + sl, a = pid % A;
+    const float* row = rpm + (size_t)sl * nL;
+    // candidate filter and the lookups that do not read the load (the rate is tested per scenario)
+    const float one = 1.0f;
+    const bool usable = is_candidate_accel(sys, s, a) && pair_lookups_ok(server_view(sys, s, &one), 0, a);
+    const long long inTok = sys.srv_in_tokens[s], Kt = sys.srv_out_tokens[s];
+    const int minRep = sys.srv_min_replicas[s];
+    const float tps = sys.srv_slo_tps[s];
+    // 0: nil or the empty record; 1: zeroLoadAllocation; 2: needs Size.  A totalRate that is NaN, or 0 on a server whose
+    // replica floor is not positive, gives the per-replica rate NaN (0 / 0 when numReplicas is 0): the reference's
+    // Analyze never returns on it (mm1modelstatedependent.go:84), so the item gets the empty record and starts no chain.
+    auto kind = [&](float r) -> int {
+        if (!usable || r < 0.0f) return 0;
+        if (r == 0.0f || Kt == 0) return 1;
+        const float totalRate = tps == 0.0f ? r / 60.0f : tps / (float)Kt;
+        return (totalRate != totalRate || (totalRate == 0.0f && minRep <= 0)) ? 0 : 2;
+    };
+    int first = nL;                                    // the first scenario that needs Size
+    for (int j = lane; j < nL; j += 32)
+        if (first == nL && kind(row[j]) == 2) first = j;
+    first = __reduce_min_sync(0xffffffffu, first);
+    const int m = sys.srv_model[s];
+    unsigned long long steps = 0, analyzed = 0;
+
+    // every scenario's record; wp, st1 (the Solve behind rateStar, at lambda x1), rateStar and N count when sized
+    auto rounds = [&](const WarpPair* wp, const SolveStats& st1, float x1, float rateStar, long long N, bool sized,
+                      bool sizeSlow) {
+        for (int j0 = 0; j0 < nL; j0 += 32) {
+            const int j = j0 + lane;
+            const float r = j < nL ? row[j] : -1.0f;
+            const int k = j < nL ? kind(r) : 0;
+            AllocRec rec = empty_alloc();
+            bool ok = false, slow = false, act = false;
+            float x = 0.0f;
+            long long numReplicas = 0;
+            float cost = 0.0f;
+            if (k == 1) { rec = zero_load_allocation(sys, s, a); ok = true; }
+            else if (k == 2 && sizeSlow) slow = true;           // the whole item is re-run with p[] in HBM
+            else if (k == 2 && sized) {
+                const float totalRate = tps == 0.0f ? r / 60.0f : tps / (float)Kt;
+                numReplicas = go_f64_to_int(ceil((double)totalRate / (double)rateStar));
+                if (numReplicas < (long long)minRep) numReplicas = minRep;
+                cost = sys.acc_cost[a] * (float)go_muli(num_instances(sys, m, a), numReplicas);
+                const float rate2 = totalRate / (float)numReplicas;
+                ++analyzed;
+                // rate2 <= 0 or above RateRange.Max: Analyze's error, nil.  A NaN rate2 (which kind() rules out) gives
+                // the empty record too, before any chain.
+                if (rate2 == rate2 && !(rate2 <= 0.0f || rate2 > wp->rateMax)) {
+                    x = rate2 / 1000.0f;
+                    act = x != x1;
+                    ok = !act;                                  // the same Solve as rateStar's
+                }
+            }
+            SolveStats st2 = st1;
+            if (__any_sync(0xffffffffu, act)) {
+                bool v, uu;
+                const bool solved = warp_solve(*wp, act, x, st2, steps, v, false, uu);
+                if (act && !solved) slow = true;
+                else if (act) ok = v;
+            }
+            if (ok && k == 2) {
+                wva_metrics m2; metrics_from(*wp, st2, m2);
+                rec.acc = a; rec.numReplicas = numReplicas; rec.batchSize = N;
+                rec.cost = cost; rec.itl = m2.avg_token_time;
+                rec.ttft = m2.avg_wait_time + m2.avg_prefill_time;
+                rec.rho = m2.rho; rec.maxArrv = rateStar / 1000.0f;
+                rec.value = cost;
+            }
+            if (ok) rec.value = transition_penalty(sys.srv_cur_acc[s], sys.srv_cur_replicas[s], sys.srv_cur_cost[s], rec.acc,
+                                                   rec.numReplicas, rec.cost);
+            if (j < nL) {
+                const unsigned long long item = ((unsigned long long)sl * nL + j) * A + a;
+                if (slow) { ok = false; slow_list[atomicAdd(slow_count, 1)] = item; }
+                if (!ok) rec = empty_alloc();
+                plane[item] = to_pair_rec(rec, ok);
+            }
+        }
+    };
+
+    bool hooked = false, sizeSlow = false;
+    if (first < nL) {
+        const size_t pi = (size_t)m * A + a;
+        long long N;
+        if (sys.srv_max_batch[s] > 0) N = sys.srv_max_batch[s];
+        else { N = go_divi(go_muli(sys.perf_max_batch[pi], sys.perf_at_tokens[pi]), Kt); if (N < 1) N = 1; }
+        if (config_ok(N, go_muli(N, WVA_MAX_QUEUE_TO_BATCH_RATIO), inTok, Kt)) {
+            if (lane == 0) atomicAdd(counters + 4, 1ull);
+            auto table = [&](WarpPair& w, long long n) -> double2* {
+                if (tabOff[pid] < 0 || n > (1LL << 26)) return nullptr;
+                double2* tab = (w.N <= smemEntriesPerWarp)
+                                   ? reinterpret_cast<double2*>(loads_smem) + (size_t)(threadIdx.x >> 5) * smemEntriesPerWarp
+                                   : tabs + tabOff[pid];
+                w.pstore = nullptr;
+                bool bad = false;
+                for (int i = lane; i < w.N; i += 32) {       // BuildModel (queueanalyzer.go:99-131)
+                    const float r = w.sv.rate(i + 1);
+                    if (!(r > 0.0f) || !(r < CUDART_INF_F)) bad = true;
+                    const double d = (double)r;
+                    tab[i] = make_double2(d, rcp_refined(d));
+                }
+                __syncwarp();
+                return __any_sync(0xffffffffu, bad) ? nullptr : tab;
+            };
+            auto atLambda = [&](const WarpPair& wp, const SolveStats& st, float lastX, float requestRate, long long n) {
+                // rateStar = Analyze(requestRate).Throughput (:237-241), from a lane's evaluation at that lambda if any
+                hooked = true;
+                const float x1 = requestRate / 1000.0f;
+                const unsigned have = __ballot_sync(0xffffffffu, lastX == x1);
+                SolveStats st1 = st;
+                bool valid1 = true, slow1 = false;
+                if (have == 0u) {
+                    SolveStats stl = st;
+                    bool v, uu;
+                    const bool solved = warp_solve(wp, lane == 0, x1, stl, steps, v, false, uu);
+                    if (__any_sync(0xffffffffu, lane == 0 && !solved)) slow1 = true;
+                    else { st1 = shfl_stats(stl, 0); valid1 = __shfl_sync(0xffffffffu, (int)v, 0); }
+                } else st1 = shfl_stats(st, __ffs(have) - 1);
+                float rateStar = 0.0f;
+                if (!slow1 && valid1) { wva_metrics m1; metrics_from(wp, st1, m1); rateStar = m1.throughput; }
+                rounds(&wp, st1, x1, rateStar, n, !slow1 && valid1, slow1);
+            };
+            AllocRec rec = empty_alloc();
+            bool ok = false;
+            int activeRounds = 0, totalRounds = 0, pendEvals = 0;
+            long long solveCycles = 0;
+            // Size does not read the rate: the server seen at its first sizing scenario serves them all
+            size_pair_warp(server_view(sys, s, row + first), 0, a, sys.srv_max_batch[s], table, lane, counters, rec, ok, sizeSlow,
+                           steps, activeRounds, totalRounds, pendEvals, solveCycles, LambdaHook<decltype(atLambda)>{atLambda});
+        }
+    }
+    if (!hooked) rounds(nullptr, SolveStats{}, -1.0f, 0.0f, 0, false, sizeSlow);     // Size failed, or needs p[] in HBM
+    for (int o = 16; o > 0; o >>= 1) {
+        steps += __shfl_down_sync(0xffffffffu, steps, o);
+        analyzed += __shfl_down_sync(0xffffffffu, analyzed, o);
+    }
+    if (lane == 0 && steps) atomicAdd(counters, steps);
+    if (lane == 0 && analyzed) atomicAdd(counters + 5, analyzed);
+}
+
+// item = ((s - s0) * nL + j) * A + a of the slice: Server.Calculate on the server seen at rate rpm[(s - s0) * nL + j],
+// p[] materialised in HBM at scratch + scratch_off[t] (11 N + 1 doubles)
+__global__ void __launch_bounds__(64)
+k_pairs_loads_literal(DevSystem sys, int s0, int nL, const float* __restrict__ rpm, const unsigned long long* __restrict__ list,
+                      int nList, double* scratch, const long long* __restrict__ scratch_off, wva_pair_rec* __restrict__ plane,
+                      unsigned long long* step_counter) {
+    int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nList) return;
+    const unsigned long long item = list[t];
+    const unsigned long long rowIdx = item / (unsigned long long)sys.A;     // (s - s0) * nL + j
+    const int a = (int)(item % (unsigned long long)sys.A), s = s0 + (int)(rowIdx / (unsigned long long)nL);
+    AllocRec rec = empty_alloc();
+    int fault = 0;
+    unsigned long long steps = 0;
+    bool ok = calculate_pair(server_view(sys, s, rpm + rowIdx), 0, a, scratch + scratch_off[t], rec, fault, steps);
+    if (!ok) rec = empty_alloc();
+    plane[item] = to_pair_rec(rec, ok);
+    atomicAdd(step_counter, steps);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -102,7 +102,44 @@ int main(void) {
         nb += r->feasible;
     }
     CHECK(nb > 0);
-    printf("cabi_test: ok (%d feasible pairs, type counts %lld %lld, %d at batch size 24)\n", nfe, (long long)cnt[0], (long long)cnt[1], nb);
+    /* pair sizing over arrival-rate scenarios: column j equals wva_pairs_fetch after an upload with that rate, and best
+     * equals wva_solve(unlimited)'s choice on that image */
+    enum { L = 3 };
+    const float fac[L] = {0.5f, 2.0f, 7.0f};
+    float rpm[S * L];
+    for (int s = 0; s < S; ++s)
+        for (int j = 0; j < L; ++j) rpm[s * L + j] = sar[s] * fac[j];
+    rpm[1 * L + 0] = -1.0f;      /* nil */
+    wva_pair_rec lplane[S * L * A], lbest[S * L];
+    CHECK(wva_analyze_pairs_loads(ctx, L, rpm, lplane, lbest) == WVA_OK);
+    uint64_t lcnt[5];
+    CHECK(wva_pairs_loads_counters(ctx, lcnt) == WVA_OK && lcnt[0] == 1 && lcnt[1] > 0 && lcnt[2] > 0);
+    CHECK(wva_analyze_pairs_loads(ctx, 0, rpm, NULL, NULL) == WVA_EINVAL && wva_analyze_pairs_loads(ctx, L, NULL, NULL, NULL) == WVA_EINVAL);
+    int nl = 0;
+    for (int j = 0; j < L; ++j) {
+        for (int s = 0; s < S; ++s) sar[s] = rpm[s * L + j];
+        CHECK(wva_system_upload(ctx, &h) == WVA_OK);
+        CHECK(wva_analyze_pairs(ctx, &o2, fe2) == WVA_OK);
+        CHECK(wva_solve(ctx, &spec, key2, &c2) == WVA_OK);
+        for (int s = 0; s < S; ++s) {
+            for (int a = 0; a < A; ++a) {
+                const int i = s * A + a;
+                const wva_pair_rec* r = &lplane[(s * L + j) * A + a];
+                CHECK(r->acc == acc2[i] && r->feasible == fe2[i] && r->num_replicas == rep2[i] && r->batch_size == bat2[i]);
+                CHECK(!memcmp(&r->cost, &f2[0][i], 4) && !memcmp(&r->value, &f2[1][i], 4) && !memcmp(&r->itl, &f2[2][i], 4));
+                CHECK(!memcmp(&r->ttft, &f2[3][i], 4) && !memcmp(&r->rho, &f2[4][i], 4) && !memcmp(&r->max_arrv_rate_per_replica, &f2[5][i], 4));
+                nl += r->feasible;
+            }
+            const wva_pair_rec* b = &lbest[s * L + j];
+            if (key2[s] < 0) { CHECK(b->acc == WVA_ACC_NONE && b->feasible == 0); continue; }
+            CHECK(b->feasible == 1 && b->acc == cacc2[s] && b->num_replicas == crep2[s] && b->batch_size == cbat2[s]);
+            CHECK(!memcmp(&b->cost, &cf2[0][s], 4) && !memcmp(&b->value, &cf2[1][s], 4) && !memcmp(&b->itl, &cf2[2][s], 4));
+            CHECK(!memcmp(&b->ttft, &cf2[3][s], 4) && !memcmp(&b->rho, &cf2[4][s], 4) && !memcmp(&b->max_arrv_rate_per_replica, &cf2[5][s], 4));
+        }
+    }
+    CHECK(nl > 0);
+    printf("cabi_test: ok (%d feasible pairs, type counts %lld %lld, %d at batch size 24, %d over %d arrival-rate scenarios)\n",
+           nfe, (long long)cnt[0], (long long)cnt[1], nb, nl, (int)L);
     wva_ctx_destroy(ctx);
     return 0;
 }
