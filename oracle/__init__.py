@@ -51,6 +51,9 @@ def lib():
         L.wvao_transition_penalty.argtypes = [C.c_int32, C.c_int64, C.c_float, C.c_int32, C.c_int64, C.c_float]
         L.wvao_queue_analyze.argtypes = [C.c_int32, C.c_void_p, abi.f32p, C.c_void_p, abi.u8p]
         L.wvao_queue_size.argtypes = [C.c_int32, C.c_void_p, abi.f32p, abi.f32p, C.c_void_p, abi.f32p, abi.u8p]
+        L.wvao_queue_size_mt.argtypes = [C.c_int32, C.c_void_p, abi.f32p, abi.f32p, C.c_void_p, abi.f32p, abi.u8p, C.c_int]
+        L.wvao_analyzer_eval.argtypes = [C.c_void_p, C.c_int, C.c_float, abi.f32p]
+        L.wvao_rescale_counts.argtypes = [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.wvao_queue_analyze_mt.argtypes = [C.c_int32, C.c_void_p, abi.f32p, C.c_void_p, abi.u8p, C.c_int]
         L.wvao_grid_candidates.argtypes = [C.POINTER(abi.SystemSoa), C.c_int64, abi.i32p, abi.i32p, abi.i32p, abi.i32p,
                                            C.c_void_p, abi.u8p, C.c_int]
@@ -87,6 +90,14 @@ def lib():
 def rescale_events():
     lib().wvao_rescale_events.restype = C.c_uint64
     return int(lib().wvao_rescale_events())
+
+
+def rescale_counts():
+    """(chain, sum): rescale branches taken since load by the chain (mm1modelstatedependent.go:84-89) and by the
+    normalising sum (:95-104); rescale_events() is their total"""
+    chain, total = C.c_uint64(), C.c_uint64()
+    lib().wvao_rescale_counts(C.byref(chain), C.byref(total))
+    return int(chain.value), int(total.value)
 
 
 def hardware_threads():
@@ -135,6 +146,12 @@ class Analyzer:
         out = np.zeros(self.K + 1, dtype=np.float64)
         lib().wvao_analyzer_probabilities(self.h, out.ctypes.data_as(C.POINTER(C.c_double)), len(out))
         return out
+
+    def eval(self, kind, x):
+        """EvalTTFT (kind 0) / EvalITL (kind 1) at lambda = x -> float32 y, or None where the model is invalid"""
+        y = C.c_float()
+        err = lib().wvao_analyzer_eval(self.h, kind, C.c_float(x), C.byref(y))
+        return None if err else np.float32(y.value)
 
     def binary_search(self, kind, x_min, x_max, y_target):
         x, ind = C.c_float(), C.c_int()
@@ -230,7 +247,7 @@ def grid_candidates(img, s, a, r, b, threads=1):
     return metrics, status
 
 
-def queue_size(cfgs, targets):
+def queue_size(cfgs, targets, threads=1):
     cfgs = np.ascontiguousarray(cfgs, dtype=abi.QUEUE_CONFIG_DTYPE)
     targets = np.ascontiguousarray(targets, dtype=np.float32).reshape(-1)
     n = len(cfgs)
@@ -238,8 +255,8 @@ def queue_size(cfgs, targets):
     achieved = np.zeros(3 * n, dtype=np.float32)
     metrics = np.zeros(n, dtype=abi.METRICS_DTYPE)
     status = np.zeros(n, dtype=np.uint8)
-    lib().wvao_queue_size(n, cfgs.ctypes.data, abi.ptr(targets, C.c_float), abi.ptr(rates, C.c_float),
-                          metrics.ctypes.data, abi.ptr(achieved, C.c_float), abi.ptr(status, C.c_uint8))
+    lib().wvao_queue_size_mt(n, cfgs.ctypes.data, abi.ptr(targets, C.c_float), abi.ptr(rates, C.c_float),
+                             metrics.ctypes.data, abi.ptr(achieved, C.c_float), abi.ptr(status, C.c_uint8), int(threads))
     return rates.reshape(n, 3), metrics, achieved.reshape(n, 3), status
 
 

@@ -71,7 +71,10 @@ inline int go_cmpf(float x, float y) {
 }
 inline int go_cmpi(int64_t x, int64_t y) { return x < y ? -1 : (x > y ? +1 : 0); }
 
-std::atomic<uint64_t> g_rescale_events{0};   // instrumentation: overflow-rescale branches taken
+// instrumentation: overflow-rescale branches taken, the chain's (mm1modelstatedependent.go:84-89) and the
+// normalising sum's (:95-104) apart
+std::atomic<uint64_t> g_rescale_chain{0};
+std::atomic<uint64_t> g_rescale_sum{0};
 const float kMaxFloat32 = std::numeric_limits<float>::max();
 const double kMaxFloat64 = std::numeric_limits<double>::max();
 
@@ -128,7 +131,7 @@ struct StateDependentModel {
             double t = p[n] * (double)lambda;                                   // :83, (p*lambda)/s
             p[n + 1] = t / sRate;
             while (p[n + 1] < 0 || std::isinf(p[n + 1]) || std::isnan(p[n + 1])) {   // :84
-                g_rescale_events++;
+                g_rescale_chain++;
                 for (int64_t i = 0; i <= n; i++) p[i] /= scale;
                 double t2 = p[n] * (double)lambda;
                 p[n + 1] = t2 / sRate;
@@ -138,7 +141,7 @@ struct StateDependentModel {
         for (int64_t n = 0; n <= K; n++) {
             sum += p[n];
             if (sum < 0 || std::isinf(sum)) {                                   // :95
-                g_rescale_events++;
+                g_rescale_sum++;
                 sum = 0;
                 for (int64_t i = 0; i <= K; i++) {
                     p[i] /= scale;
@@ -744,21 +747,25 @@ int wvao_queue_analyze(int32_t n, const wva_queue_config* cfg, const float* rate
     return wvao_queue_analyze_mt(n, cfg, rate, metrics, status, 1);
 }
 
-int wvao_queue_size(int32_t n, const wva_queue_config* cfg, const float* target, float* rates, wva_metrics* metrics,
-                    float* achieved, uint8_t* status) {
-    for (int32_t i = 0; i < n; i++) {
+int wvao_queue_size_mt(int32_t n, const wva_queue_config* cfg, const float* target, float* rates, wva_metrics* metrics,
+                       float* achieved, uint8_t* status, int threads) {
+    parallelFor(n, threads, [&](int64_t i) {
         std::memset(&metrics[i], 0, sizeof(wva_metrics));
         for (int k = 0; k < 3; k++) { rates[3 * i + k] = 0; achieved[3 * i + k] = 0; }
         const wva_queue_config& c = cfg[i];
-        if (!configOk(c.max_batch_size, c.max_queue_size, c.avg_input_tokens, c.avg_output_tokens)) { status[i] = 1; continue; }
+        if (!configOk(c.max_batch_size, c.max_queue_size, c.avg_input_tokens, c.avg_output_tokens)) { status[i] = 1; return; }
         QueueAnalyzer qa;
         buildModel(qa, c.max_batch_size, c.max_queue_size, ServiceParms{c.alpha, c.beta, c.gamma, c.delta},
                    c.avg_input_tokens, c.avg_output_tokens);
         bool ok = sizeQueue(qa, target[3 * i], target[3 * i + 1], target[3 * i + 2], &rates[3 * i], &metrics[i], &achieved[3 * i]);
         if (!ok) { std::memset(&metrics[i], 0, sizeof(wva_metrics)); for (int k = 0; k < 3; k++) { rates[3 * i + k] = 0; achieved[3 * i + k] = 0; } }
         status[i] = ok ? 0 : 1;
-    }
+    });
     return WVA_OK;
+}
+int wvao_queue_size(int32_t n, const wva_queue_config* cfg, const float* target, float* rates, wva_metrics* metrics,
+                    float* achieved, uint8_t* status) {
+    return wvao_queue_size_mt(n, cfg, target, rates, metrics, achieved, status, 1);
 }
 
 // A persistent analyzer handle so tests can exercise the stale-p[0] validity state
@@ -842,6 +849,11 @@ float wvao_effective_concurrency(float servTime, float alpha, float beta, float 
 // analyzer.BinarySearch on the model (utils.go:26-70) with EvalTTFT (kind 0) / EvalITL (kind 1)
 int wvao_analyzer_binary_search(wvao_analyzer* h, int kind, float xMin, float xMax, float yTarget, float* x, int* ind) {
     return binarySearch(h->qa, kind == 0 ? EVAL_TTFT : EVAL_ITL, xMin, xMax, yTarget, x, ind) ? 0 : 1;
+}
+// EvalTTFT (kind 0) / EvalITL (kind 1) at x on the handle's model: 0 and *y, or 1 for "invalid model"
+int wvao_analyzer_eval(wvao_analyzer* h, int kind, float x, float* y) {
+    *y = 0;
+    return evalTarget(h->qa, kind == 0 ? EVAL_TTFT : EVAL_ITL, x, y) ? 0 : 1;
 }
 int wvao_within_tolerance(float x, float v, float tol) { return withinTolerance(x, v, tol) ? 1 : 0; }
 float wvao_transition_penalty(int32_t aAcc, int64_t aRep, float aCost, int32_t bAcc, int64_t bRep, float bCost) {
@@ -1092,7 +1104,9 @@ int wvao_allocate_by_type(const wva_system_soa* sys, int32_t s0, int32_t s1, con
 }
 
 // number of overflow-rescale branches (mm1modelstatedependent.go:84-89, :96-104) taken since load
-uint64_t wvao_rescale_events(void) { return g_rescale_events.load(); }
+uint64_t wvao_rescale_events(void) { return g_rescale_chain.load() + g_rescale_sum.load(); }
+// the same, per branch: the chain's (:84-89) and the normalising sum's (:95-104)
+void wvao_rescale_counts(uint64_t* chain, uint64_t* sum) { *chain = g_rescale_chain.load(); *sum = g_rescale_sum.load(); }
 
 int wvao_hardware_threads(void) { unsigned n = std::thread::hardware_concurrency(); return n ? (int)n : 1; }
 
