@@ -447,7 +447,8 @@ int wva_type_totals_device(wva_ctx* ctx, void** dev_ptr, size_t* bytes);
 /* Sharded runs with a HOST-driven collective (no wva_comm_init): every rank all-gathers its 12*T-byte
  * totals block (ONE collective); this call then sums the n_ranks gathered blocks (device memory,
  * rank-major) in rank order into the totals buffer -- one launch, and unlike a ring/tree all-reduce the
- * float32 cost sums come out the same on every rank and every run.
+ * float32 cost sums come out the same on every rank and every run.  Blocks are packed back to back, so
+ * with an odd T every other block's counts are only 4-byte aligned; gathered_dev itself needs 4 bytes.
  * Ordering contract: the merge kernel is enqueued on wva_stream(ctx); the caller's collective must
  * have been enqueued on that same stream (or have completed) before this call. */
 int wva_type_totals_merge(wva_ctx* ctx, const void* gathered_dev, int32_t n_ranks);

@@ -2271,18 +2271,21 @@ __global__ void __launch_bounds__(1024) k_totals(DevSystem sys, int s0, int ns, 
 }
 
 // Sum the per-rank partial totals of a sharded run in rank order (deterministic, unlike a ring or
-// tree all-reduce): gathered = n_ranks blocks of { long long count[T]; float cost[T] }.
+// tree all-reduce): gathered = n_ranks blocks of { long long count[T]; float cost[T] }.  A block is
+// 12*T bytes, so with T odd every odd rank's counts sit 4 bytes off an 8-byte boundary: they are read
+// as two 32-bit words (little-endian) and summed as unsigned, which wraps like Go's int64.
 __global__ void k_totals_merge(int T, int n_ranks, const unsigned char* __restrict__ gathered, long long* __restrict__ count,
                                float* __restrict__ cost) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
-    long long c = 0; float k = 0.0f;
+    unsigned long long c = 0; float k = 0.0f;
     for (int r = 0; r < n_ranks; ++r) {
         const unsigned char* blk = gathered + (size_t)r * T * 12;
-        c += reinterpret_cast<const long long*>(blk)[t];
+        const unsigned* w = reinterpret_cast<const unsigned*>(blk) + 2 * (size_t)t;
+        c += (unsigned long long)w[0] | ((unsigned long long)w[1] << 32);
         k = k + reinterpret_cast<const float*>(blk + (size_t)T * 8)[t];
     }
-    count[t] = c; cost[t] = k;
+    count[t] = (long long)c; cost[t] = k;
 }
 
 // pkg/analyzer's bare model: a sequence of MM1ModelStateDependent.Solve(lambda, mu) calls on ONE model instance

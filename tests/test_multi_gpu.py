@@ -27,6 +27,8 @@ def _worker(rank, world, port, q):
     wva = wva_import.load()
     from inferno_autoscaler_b200 import binding, distributed as D
     import oracle
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import rank_emulation
     dev = torch.device("cuda", rank)
     img = wva.synth.make_system(61, 4, seed=93, n_types=2, max_pair_batch=128)
     pairs_all, feas_all, _ = oracle.analyze_pairs(img, threads=4)
@@ -42,8 +44,8 @@ def _worker(rank, world, port, q):
     ctx.allocate_by_type()
     cnt, cst = D.allreduce_totals_device(ctx, img.T, dev)
     torch.cuda.synchronize()
-    w_cnt, w_cst = oracle.allocate_by_type(img, acc_u, ch_u)
-    ok = ok and np.array_equal(cnt.cpu().numpy(), w_cnt) and np.allclose(cst.cpu().numpy(), w_cst, rtol=1e-5)
+    w_cnt, w_cst = rank_emulation.expected_totals(oracle, img, acc_u, ch_u, world)     # rank-order sum of the shard partials
+    ok = ok and np.array_equal(cnt.cpu().numpy(), w_cnt) and cst.cpu().numpy().tobytes() == w_cst.tobytes()
     ok = ok and np.array_equal(acc[first:first + count], acc_u[first:first + count])
     # limited: gather rows in place, identical greedy everywhere
     ctx.upload(img); ctx.set_shard(first, count)
@@ -56,8 +58,8 @@ def _worker(rank, world, port, q):
     ctx.allocate_by_type()
     cnt, cst = D.allreduce_totals_device(ctx, img.T, dev)
     torch.cuda.synchronize()
-    w_cnt, w_cst = oracle.allocate_by_type(img, w_acc, w_chosen)
-    ok = ok and np.array_equal(cnt.cpu().numpy(), w_cnt) and np.allclose(cst.cpu().numpy(), w_cst, rtol=1e-5)
+    w_cnt, w_cst = rank_emulation.expected_totals(oracle, img, w_acc, w_chosen, world)
+    ok = ok and np.array_equal(cnt.cpu().numpy(), w_cnt) and cst.cpu().numpy().tobytes() == w_cst.tobytes()
     # ---- the same two modes with the collective inside the library --------------------------------
     D.attach_library_comm(ctx, dev)
     ctx.upload(img); ctx.comm_shard()
@@ -65,8 +67,8 @@ def _worker(rank, world, port, q):
     ctx.analyze_pairs(download=False)
     acc, chosen = ctx.solve(unlimited=True)
     cnt, cst = ctx.allocate_by_type()                       # GLOBAL totals, exchanged by the library
-    w_cnt, w_cst = oracle.allocate_by_type(img, acc_u, ch_u)
-    ok = ok and np.array_equal(cnt, w_cnt) and np.allclose(cst, w_cst, rtol=1e-5)
+    w_cnt, w_cst = rank_emulation.expected_totals(oracle, img, acc_u, ch_u, world)
+    ok = ok and np.array_equal(cnt, w_cnt) and cst.tobytes() == w_cst.tobytes()
     ok = ok and np.array_equal(acc[first:first + count], acc_u[first:first + count])
     box = [cst.tobytes()]
     dist.broadcast_object_list(box, src=0)
@@ -78,8 +80,8 @@ def _worker(rank, world, port, q):
         w_acc, w_chosen = oracle.solve(img, pairs_all, feas_all, unlimited=False, policy=policy)
         ok = ok and np.array_equal(acc, w_acc) and chosen.equal_bits(w_chosen)[0]
         cnt, cst = ctx.allocate_by_type()
-        w_cnt, w_cst = oracle.allocate_by_type(img, w_acc, w_chosen)
-        ok = ok and np.array_equal(cnt, w_cnt) and np.allclose(cst, w_cst, rtol=1e-5)
+        w_cnt, w_cst = rank_emulation.expected_totals(oracle, img, w_acc, w_chosen, world)
+        ok = ok and np.array_equal(cnt, w_cnt) and cst.tobytes() == w_cst.tobytes()
     q.put((rank, bool(ok)))
     ctx.comm_destroy()
     ctx.close()
@@ -105,6 +107,8 @@ def _group_case(n_dev):
     wva = wva_import.load()
     from inferno_autoscaler_b200 import binding
     import oracle
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import rank_emulation
     img = wva.synth.make_system(61, 4, seed=93, n_types=2, max_pair_batch=128)
     pairs_all, feas_all, _ = oracle.analyze_pairs(img, threads=4)
     acc_u, ch_u = oracle.solve(img, pairs_all, feas_all, unlimited=True)
@@ -121,10 +125,8 @@ def _group_case(n_dev):
         acc, chosen = g.solve(unlimited=True)
         assert np.array_equal(acc, acc_u) and chosen.equal_bits(ch_u)[0]
         cnt, cst = g.allocate_by_type()
-        w_cnt, w_cst = oracle.allocate_by_type(img, acc_u, ch_u)
-        assert np.array_equal(cnt, w_cnt) and np.allclose(cst, w_cst, rtol=1e-5)
-        if n_dev == 1:
-            assert cst.tobytes() == w_cst.tobytes()
+        w_cnt, w_cst = rank_emulation.expected_totals(oracle, img, acc_u, ch_u, n_dev)   # rank-order sum of the shard partials
+        assert np.array_equal(cnt, w_cnt) and cst.tobytes() == w_cst.tobytes()
         for policy in (wva.abi.POLICY_NONE, wva.abi.POLICY_ROUND_ROBIN):
             g.upload(img)
             g.analyze()
@@ -132,8 +134,8 @@ def _group_case(n_dev):
             w_acc, w_chosen = oracle.solve(img, pairs_all, feas_all, unlimited=False, policy=policy)
             assert np.array_equal(acc, w_acc) and chosen.equal_bits(w_chosen)[0]
             cnt, cst = g.allocate_by_type()
-            w_cnt, w_cst = oracle.allocate_by_type(img, w_acc, w_chosen)
-            assert np.array_equal(cnt, w_cnt) and np.allclose(cst, w_cst, rtol=1e-5)
+            w_cnt, w_cst = rank_emulation.expected_totals(oracle, img, w_acc, w_chosen, n_dev)
+            assert np.array_equal(cnt, w_cnt) and cst.tobytes() == w_cst.tobytes()
             assert (cnt <= img.type_capacity).all()
     finally:
         g.close()
