@@ -181,7 +181,8 @@ int  wva_abi_version(void);
 
 /* Replaces core.NewSystem + System.SetFromSpec (pkg/core/system.go:67-90) and the
  * manager.NewManager side effect core.TheSystem = system (pkg/manager/manager.go:13-19).
- * Uploads the image to HBM; invalidates previous analysis. */
+ * Uploads the image to HBM; invalidates previous analysis and resets the shard to its default (see
+ * wva_set_shard). */
 int wva_system_upload(wva_ctx* ctx, const wva_system_soa* host);
 
 /* Incremental updates of the RESIDENT image (System.AddServerFromSpec / RemoveServer / SetCountFromSpec /
@@ -189,7 +190,7 @@ int wva_system_upload(wva_ctx* ctx, const wva_system_soa* host);
  * wva_system_upload lays the arrays out with spare rows (1/16 more, at least 64); an update that would
  * outgrow them fails with WVA_ECAPACITY and the caller uploads the whole image again.  Every update that
  * changes rows invalidates previous analysis results (pair records, decisions, sweep results) and resets the
- * shard to "everything".  An update that fails changes nothing: image, dimensions, shard, wva_upload_bytes and
+ * shard to its default (see wva_set_shard).  An update that fails changes nothing: image, dimensions, shard, wva_upload_bytes and
  * results stay as they were.  A zero-row update (count == 0, after the same argument checks) is a no-op that
  * keeps results and shard; wva_upload_bytes then reports 0.
  *   wva_system_update_servers: overwrite server rows [first, first+count) from rows->srv_* (arrays of
@@ -233,7 +234,13 @@ int wva_solve_arrays(wva_ctx* ctx, int32_t unlimited, int32_t delayed_best_effor
 
 /* Multi-GPU sharding (SURVEY 8e): this rank owns servers [first, first+count) of the
  * uploaded image; analysis kernels touch only those; solve/allocate_by_type produce the
- * rank's partial results.  Default shard = everything. */
+ * rank's partial results.  Default shard, which wva_system_upload and every row-changing update restore:
+ * everything without a communicator, the rank's wva_comm_shard range with one.
+ * With a communicator attached the shards of all ranks must cover every server exactly once before a limited
+ * wva_solve: a gap or an overlap between them fails that solve with WVA_EINVAL on every rank.  A shard of more
+ * than ceil(S / ranks) servers fails it with WVA_EINVAL on that rank alone, before the collective, while the
+ * other ranks' streams wait for it inside the all-gather: the caller must not get there (wva_comm_shard never
+ * does). */
 int wva_set_shard(wva_ctx* ctx, int32_t first_server, int32_t count);
 /* The shard the following calls work on: servers [*first, *first + *count).  WVA_ESTATE before any upload. */
 int wva_shard_info(const wva_ctx* ctx, int32_t* first, int32_t* count);
@@ -480,7 +487,7 @@ int wva_comm_unique_id(void* id_out /* WVA_COMM_ID_BYTES */);
 int wva_comm_init(wva_ctx* ctx, const void* id, int32_t rank, int32_t n_ranks);
 int wva_comm_destroy(wva_ctx* ctx);
 int wva_comm_info(const wva_ctx* ctx, int32_t* rank, int32_t* n_ranks);   /* 0 / 1 without a communicator */
-int wva_comm_shard(wva_ctx* ctx);
+int wva_comm_shard(wva_ctx* ctx);   /* [floor(S*g/G), floor(S*(g+1)/G)); upload and updates restore it */
 
 /* (2) ONE process driving several GPUs -- the shape of the reference's caller, a single reconcile
  *     goroutine (internal/controller/variantautoscaling_controller.go:143-166).  A group owns one ctx

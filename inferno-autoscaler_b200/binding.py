@@ -211,7 +211,7 @@ class Context:
         s = image.c_struct()
         self._ck(lib().wva_system_upload(self._h, C.byref(s)))
         self.image = image
-        self.first, self.count = 0, image.S
+        self._read_shard()
 
     # ---- incremental updates of the resident image (system.go:99-171) ------------------------
     def update_servers(self, first, rows: SystemImage):
@@ -229,7 +229,7 @@ class Context:
             arr[first:first + rows.S] = getattr(rows, name)
             setattr(img, name, arr)
         img.S = newS
-        self.first, self.count = 0, newS
+        self._read_shard()
 
     def update_models(self, first, rows: SystemImage):
         s = rows.c_struct()
@@ -245,7 +245,7 @@ class Context:
             arr[first * img.A:(first + rows.M) * img.A] = getattr(rows, name)
             setattr(img, name, arr)
         img.M = newM
-        self.first, self.count = 0, img.S
+        self._read_shard()
 
     def remove_server(self, index):
         """RemoveServer: the last server's row moves into `index`; self.image follows"""
@@ -256,7 +256,7 @@ class Context:
             arr[index] = arr[img.S - 1]
             setattr(img, name, arr[:img.S - 1].copy())
         img.S -= 1
-        self.first, self.count = 0, img.S
+        self._read_shard()
 
     def set_capacity(self, type_capacity):
         cap = np.ascontiguousarray(type_capacity, dtype=np.int64)
@@ -270,6 +270,12 @@ class Context:
         v = [C.c_int32(0) for _ in range(4)]
         self._ck(lib().wva_system_dims(self._h, *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
+
+    def _read_shard(self):
+        """the library's shard after an upload or update: everything, or the communicator range with one attached"""
+        f, n = C.c_int32(0), C.c_int32(0)
+        self._ck(lib().wva_shard_info(self._h, C.byref(f), C.byref(n)))
+        self.first, self.count = f.value, n.value
 
     def set_shard(self, first, count):
         self._ck(lib().wva_set_shard(self._h, int(first), int(count)))

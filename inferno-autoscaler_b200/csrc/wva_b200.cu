@@ -306,8 +306,19 @@ cudaError_t download_allocs(wva_ctx* ctx, const DevAllocs& d, size_t first, size
     return cudaSuccess;
 }
 
+// The shard an upload or a row-changing update leaves: with a communicator attached the rank's range
+// [floor(S*g/G), floor(S*(g+1)/G)) (what wva_comm_shard gives), without one every server.
+void reset_shard(wva_ctx* ctx) {
+    const long long S = ctx->S, g = ctx->comm ? ctx->comm_rank : 0, G = ctx->comm ? ctx->comm_size : 1;
+    ctx->s0 = (int)(S * g / G);
+    ctx->ns = (int)(S * (g + 1) / G) - ctx->s0;
+}
+
 // limited mode with a communicator: every rank packs the candidate records of its shard into one chunk,
-// ONE ncclAllGather moves all chunks, the other ranks' rows are scattered into place.
+// ONE ncclAllGather moves all chunks, the other ranks' rows are scattered into place.  Every rank reads the
+// G chunk headers {first, n} back and scatters only when the shards tile [0, S*A) exactly: all ranks hold
+// the same headers, so they reach the same verdict without another collective, and a gap or an overlap
+// is an error on every rank instead of a greedy over rows nobody sized.
 int comm_gather_pairs(wva_ctx* ctx) {
     const NcclApi& nc = nccl_api();
     if (!nc.ok) return fail(ctx, WVA_ECUDA, "NCCL unavailable: " + nc.err);
@@ -324,6 +335,21 @@ int comm_gather_pairs(wva_ctx* ctx) {
     LAUNCH_CHECK();
     int nrc = nc.AllGather(ctx->commChunk.p, ctx->commGather.p, chunkBytes, kNcclChar, ctx->comm, ctx->stream);
     if (nrc != 0) return fail(ctx, WVA_ECUDA, std::string("ncclAllGather(pairs): ") + nc.GetErrorString(nrc));
+    std::vector<int> hdr((size_t)G * 4);
+    CK(cudaMemcpy2DAsync(hdr.data(), 16, ctx->commGather.p, chunkBytes, 16, (size_t)G, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::vector<std::pair<long long, long long>> parts;    // {first pair, pairs} of every non-empty shard
+    for (int r = 0; r < G; ++r)
+        if (hdr[(size_t)r * 4 + 1] != 0) parts.emplace_back(hdr[(size_t)r * 4], hdr[(size_t)r * 4 + 1]);
+    std::sort(parts.begin(), parts.end());
+    long long end = 0;
+    bool tiled = true;
+    for (const auto& p : parts) {
+        tiled = tiled && p.first == end;
+        end += p.second;
+    }
+    if (!tiled || end != (long long)ctx->S * A)
+        return fail(ctx, WVA_EINVAL, "the ranks' shards do not cover every server exactly once: use wva_comm_shard for the limited-capacity exchange");
     dim3 grid((unsigned)((cap + 255) / 256 < 1024 ? (cap + 255) / 256 : 1024), (unsigned)G);
     k_pairs_unpack<<<grid, 256, 0, ctx->stream>>>(ctx->commGather.as<unsigned char>(), chunkBytes, cap, ctx->comm_rank, (size_t)ctx->S * A,
                                                    ctx->pairs, ctx->feasible);
@@ -533,7 +559,7 @@ int wva_system_upload(wva_ctx* ctx, const wva_system_soa* h) {
     ds.srv_priority = (const int*)(d + o_spr); ds.srv_min_replicas = (const int*)(d + o_smr); ds.srv_max_batch = (const int*)(d + o_smb); ds.srv_keep_acc = (const unsigned char*)(d + o_ska);
     ds.srv_cur_acc = (const int*)(d + o_sca); ds.srv_cur_replicas = (const int*)(d + o_scr); ds.srv_cur_cost = (const float*)(d + o_scc);
     ctx->S = S; ctx->A = A; ctx->M = M; ctx->T = T;
-    ctx->s0 = 0; ctx->ns = S;
+    reset_shard(ctx);
     // host copies of what sizes the pair tables
     ctx->h_srv_model.assign(h->srv_model, h->srv_model + S); ctx->h_srv_out.assign(h->srv_out_tokens, h->srv_out_tokens + S);
     ctx->h_srv_mb.assign(h->srv_max_batch, h->srv_max_batch + S); ctx->h_srv_arr.assign(h->srv_arrival_rpm, h->srv_arrival_rpm + S);
@@ -2125,9 +2151,8 @@ int wva_comm_info(const wva_ctx* ctx, int32_t* rank, int32_t* n_ranks) {
 int wva_comm_shard(wva_ctx* ctx) {
     if (!ctx) return WVA_EINVAL;
     if (!ctx->have_system) return fail(ctx, WVA_ESTATE, "no system uploaded");
-    const long long S = ctx->S, g = ctx->comm ? ctx->comm_rank : 0, G = ctx->comm ? ctx->comm_size : 1;
-    const int first = (int)(S * g / G), last = (int)(S * (g + 1) / G);
-    return wva_set_shard(ctx, first, last - first);
+    reset_shard(ctx);
+    return wva_set_shard(ctx, ctx->s0, ctx->ns);
 }
 
 }  // extern "C"
@@ -2331,7 +2356,7 @@ int wva_solve_arrays(wva_ctx* ctx, int32_t unlimited, int32_t delayed_best_effor
 // ---------------------------------------------------------------------------------------------
 namespace {
 void invalidate_after_update(wva_ctx* ctx) {
-    ctx->s0 = 0; ctx->ns = ctx->S;
+    reset_shard(ctx);
     ctx->dsys.S = ctx->S; ctx->dsys.M = ctx->M;
     ctx->plan_valid = false;
     ctx->pairs_valid = ctx->pairs_complete = ctx->solved = ctx->grid_valid = false;
