@@ -348,6 +348,47 @@ func (c *Context) PairsAtArrivalRates(rpm []float32, nLoads int, wantPlane bool)
 		"wva_analyze_pairs_loads")
 }
 
+// CapacityScenarios is what SolveAtCapacities returns for nVec capacity vectors: Acc[j*S+s] and Chosen[j*S+s] are the
+// limited solve's decision and chosen record (after best-effort scaling, Feasible = 1 where Acc >= 0) under vector j,
+// Count[j*T+t] and Cost[j*T+t] its AllocateByType totals over every server.
+type CapacityScenarios struct {
+	Acc    []int32
+	Chosen []PairRec
+	Count  []int64
+	Cost   []float32
+}
+
+func solveCapacitiesArgs(S, T C.int32_t, capacity []int64, nVec int) (*CapacityScenarios, error) {
+	if nVec < 1 || len(capacity) != nVec*int(T) {
+		return nil, fmt.Errorf("SolveAtCapacities: capacity needs nVec*T = %d*%d counts, got %d", nVec, int(T), len(capacity))
+	}
+	return &CapacityScenarios{Acc: make([]int32, nVec*int(S)), Chosen: make([]PairRec, nVec*int(S)),
+		Count: make([]int64, nVec*int(T)), Cost: make([]float32, nVec*int(T))}, nil
+}
+
+// SolveAtCapacities runs the limited solve once per capacity vector -- capacity[j*T .. j*T+T) is vector j, 1 <= nVec
+// <= 8192 -- on the current pair records in one call: vector j gives what SetCapacity, a limited Solve and
+// AllocateByType would.  The candidate order is built once; the pair records, the image's capacities and the last
+// Solve's decisions are left as they were, so a later limited Solve needs no re-analysis.
+func (c *Context) SolveAtCapacities(capacity []int64, nVec int, delayedBestEffort bool, policy int) (*CapacityScenarios, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var S, A, M, T C.int32_t
+	if err := c.err(C.wva_system_dims(c.ctx, &S, &A, &M, &T), "wva_system_dims"); err != nil {
+		return nil, err
+	}
+	out, err := solveCapacitiesArgs(S, T, capacity, nVec)
+	if err != nil {
+		return nil, err
+	}
+	spec := C.wva_optimizer_spec{unlimited: 0, delayed_best_effort: 0, saturation_policy: C.int32_t(policy)}
+	if delayedBestEffort {
+		spec.delayed_best_effort = 1
+	}
+	return out, c.err(C.wva_solve_capacities(c.ctx, &spec, C.int32_t(nVec), i64p(capacity), i32p(out.Acc), pairRecs(out.Chosen),
+		i64p(out.Count), f32p(out.Cost)), "wva_solve_capacities")
+}
+
 // QueueConfig is wva_queue_config; Metrics is wva_metrics (analyzer.AnalysisMetrics).
 type QueueConfig struct {
 	MaxBatchSize, MaxQueueSize int32
@@ -509,6 +550,26 @@ func (g *Group) PairsAtArrivalRates(rpm []float32, nLoads int, wantPlane bool) (
 	}
 	return plane, best, g.err(C.wva_group_analyze_pairs_loads(g.g, C.int32_t(nLoads), f32p(rpm), pairRecs(plane), pairRecs(best)),
 		"wva_group_analyze_pairs_loads")
+}
+
+// SolveAtCapacities: Context.SolveAtCapacities on every device's gathered rows; device 0 returns the results.
+func (g *Group) SolveAtCapacities(capacity []int64, nVec int, delayedBestEffort bool, policy int) (*CapacityScenarios, error) {
+	g.mu.Lock()
+	defer g.mu.Unlock()
+	var S, A, M, T C.int32_t
+	if rc := C.wva_system_dims(C.wva_group_ctx(g.g, 0), &S, &A, &M, &T); rc != C.WVA_OK {
+		return nil, fmt.Errorf("wva_system_dims: %d", int(rc))
+	}
+	out, err := solveCapacitiesArgs(S, T, capacity, nVec)
+	if err != nil {
+		return nil, err
+	}
+	spec := C.wva_optimizer_spec{unlimited: 0, delayed_best_effort: 0, saturation_policy: C.int32_t(policy)}
+	if delayedBestEffort {
+		spec.delayed_best_effort = 1
+	}
+	return out, g.err(C.wva_group_solve_capacities(g.g, &spec, C.int32_t(nVec), i64p(capacity), i32p(out.Acc), pairRecs(out.Chosen),
+		i64p(out.Count), f32p(out.Cost)), "wva_group_solve_capacities")
 }
 
 // AllocateByType: global per-type totals (NCCL all-gather of the partials inside the library).

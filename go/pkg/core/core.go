@@ -543,6 +543,16 @@ func (s *System) Solve(spec *config.OptimizerSpec) (solutionTimeUsec int64, err 
 	return usec, nil
 }
 
+// SolveAtCapacities runs the limited solve of spec under each of nVec capacity vectors (capacity[j*T+t]: vector j's count
+// of the t-th accelerator type of the uploaded image) in one native call.  Server allocations, the candidates and the
+// system's capacities are left as they were.
+func (s *System) SolveAtCapacities(spec *config.OptimizerSpec, capacity []int64, nVec int) (*native.CapacityScenarios, error) {
+	if err := s.analyzeAll(); err != nil {
+		return nil, err
+	}
+	return s.ctx.SolveAtCapacities(capacity, nVec, spec.DelayedBestEffort, int(config.SaturatedAllocationPolicyEnum(spec.SaturationPolicy)))
+}
+
 // AllocateByType (system.go:271-300)
 func (s *System) AllocateByType() {
 	s.allocationByType = map[string]*AllocationByType{}

@@ -6,6 +6,7 @@ package solver
 import (
 	"fmt"
 
+	"github.com/llm-d-incubation/workload-variant-autoscaler/go/internal/native"
 	"github.com/llm-d-incubation/workload-variant-autoscaler/go/pkg/core"
 	"github.com/llm-d-incubation/workload-variant-autoscaler/pkg/config"
 )
@@ -49,6 +50,14 @@ func (s *Solver) SolveUnlimited() { spec := *s.optimizerSpec; spec.Unlimited = t
 func (s *Solver) SolveGreedy()    { spec := *s.optimizerSpec; spec.Unlimited = false; _, _ = core.TheSystem.Solve(&spec) }
 // AllocationDiff (solver.go:81): the reference's return type.
 func (s *Solver) AllocationDiff() map[string]*core.AllocationDiff { return s.diffAllocation }
+
+// SolveAtCapacities answers "what would SolveGreedy decide under these capacities?" for nVec capacity vectors at once
+// (capacity[j*T+t]: vector j, accelerator type t of the system) without changing the system's allocations or capacities.
+func (s *Solver) SolveAtCapacities(capacity []int64, nVec int) (*native.CapacityScenarios, error) {
+	spec := *s.optimizerSpec
+	spec.Unlimited = false
+	return core.TheSystem.SolveAtCapacities(&spec, capacity, nVec)
+}
 
 type Optimizer struct {
 	spec             *config.OptimizerSpec

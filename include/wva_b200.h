@@ -438,6 +438,43 @@ int wva_solve_greedy_path(const wva_ctx* ctx);
  * from shared-group stacks << 32, SM cycles in the pass, SM cycles in bestEffort}. */
 int wva_solve_stats(wva_ctx* ctx, uint64_t out[4]);
 
+/* Limited-capacity solve over a list of capacity vectors: capacity[j * T .. j * T + T) is vector j, 1 <= n_c <= 8192.
+ * Vector j's outputs are what this library returns after wva_system_set_capacity(capacity + j * T), then a limited
+ * wva_solve(spec) on the current pair records, then wva_solution_fetch and wva_allocate_by_type:
+ *   chosen_acc [n_c * S], index j * S + s, or NULL: the solve's chosen_acc;
+ *   chosen     [n_c * S], or NULL: the solve's chosen record after best-effort scaling (greedy.go:208-212, :302-311) with
+ *              feasible = 1 where chosen_acc >= 0; elsewhere the empty record wva_solution_fetch gives (acc = -1,
+ *              feasible = 0, pad = 0);
+ *   type_count / type_cost [n_c * T], index j * T + t, or NULL: AllocateByType over ALL S servers, the float32 cost summed
+ *              in ascending server index from +0.  That is wva_allocate_by_type's sum on a context that holds every
+ *              server; a sharded context returns the same all-S ascending sums (equal on every rank), where its own
+ *              wva_allocate_by_type would merge per-shard partials in rank order (which can differ in the last float32 bits).
+ * Same semantics as wva_solve in limited mode: every saturation policy, both best-effort schedules, negative
+ * capacities, wrapped int64 counts, NaN / +-Inf values, T <= 256, every solver path (wva_solve_set_ranked).  The
+ * candidate order, the sorted static order and its event records do not depend on the capacities and are built once per
+ * call; the scan pass then runs once per vector, one warp each, side by side.  Shapes the scan path does not take, and
+ * wva_solve_set_ranked < 2, run the ranked-queue or heap kernel once per vector instead (slower, same results).  Vectors
+ * are staged in chunks whose scratch and output records fit 2^28 bytes (one vector at least); each chunk is copied out
+ * before the next starts.
+ * Nothing that other calls read changes: the resident pair records and feasible flags, whether they are valid, the
+ * image's type_capacity, the last wva_solve's decisions and whether it ran, wva_solve_greedy_path and wva_solve_stats,
+ * the totals buffer and sweep results -- a limited wva_solve right after this call needs no new wva_analyze_pairs.
+ * Errors, which change nothing: WVA_EINVAL for spec == NULL, spec->unlimited != 0 (unlimited decisions do not depend on
+ * capacities), n_c out of range, capacity == NULL, T > 256 or S * A >= 2^31; WVA_ESTATE when the pair records are not
+ * valid (no wva_analyze_pairs since the last upload, update or limited wva_solve) or when a sharded context without a
+ * communicator lacks rows (wva_solve's rule).  With a communicator and incomplete rows the call first all-gathers them
+ * as wva_solve does (one pair all-gather; none once the rows are complete). */
+#define WVA_SOLVE_MAX_CAPACITIES 8192
+int wva_solve_capacities(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n_c, const int64_t* capacity, int32_t* chosen_acc,
+                         wva_pair_rec* chosen, int64_t* type_count, float* type_cost);
+/* Counters of the last wva_solve_capacities: {vector chunks, solver path run (3 scan, 2 ranked queue, 1 heap, 0 when
+ * S = 0; as wva_solve_greedy_path), events in the static order (scan path, else 0), SM cycles of the slowest vector's
+ * pass (scan path, else 0)}. */
+int wva_solve_capacities_counters(const wva_ctx* ctx, uint64_t out[4]);
+/* Test hook: staging budget of wva_solve_capacities in bytes (0 restores the default 2^28), so that small images can
+ * span several chunks.  Results do not depend on it. */
+int wva_solve_capacities_set_budget(wva_ctx* ctx, int64_t bytes);
+
 /* Replaces System.AllocateByType (pkg/core/system.go:271-300): per accelerator type
  * count += replicas*numInstances*multiplicity, cost += alloc.cost over this rank's shard.
  * The sums are left in a device buffer (wva_type_totals_device) so the host can run the
@@ -510,6 +547,9 @@ int wva_group_analyze_pairs_loads(wva_group* g, int32_t n_l, const float* arriva
 int wva_group_analyze_pairs_batches(wva_group* g, int32_t n_b, const int32_t* batch,
                                     wva_pair_rec* plane /* [S*A*n_b] */, wva_pair_rec* best /* [S] */);   /* assembled */
 int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen);
+int wva_group_solve_capacities(wva_group* g, const wva_optimizer_spec* spec, int32_t n_c, const int64_t* capacity,
+                               int32_t* chosen_acc /* [n_c*S] */, wva_pair_rec* chosen /* [n_c*S] */, int64_t* type_count /* [n_c*T] */,
+                               float* type_cost /* [n_c*T] */);   /* every member runs it on its gathered rows; member 0 returns the results */
 int wva_group_allocate_by_type(wva_group* g, int64_t* count, float* cost);
 
 /* ---- low-level analyzer API (pkg/analyzer public surface) ------------------ */

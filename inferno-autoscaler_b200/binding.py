@@ -33,6 +33,7 @@ EXPORTS = [
     "wva_group_grid_best_blocking",
     "wva_analyze_pairs_batches", "wva_pairs_batches_counters", "wva_group_analyze_pairs_batches", "wva_shard_info",
     "wva_analyze_pairs_loads", "wva_pairs_loads_counters", "wva_group_analyze_pairs_loads",
+    "wva_solve_capacities", "wva_solve_capacities_counters", "wva_solve_capacities_set_budget", "wva_group_solve_capacities",
 ]
 
 
@@ -140,6 +141,10 @@ def lib():
         L.wva_analyze_pairs_loads.argtypes = [vp, i32, abi.f32p, vp, vp]
         L.wva_pairs_loads_counters.argtypes = [vp, C.POINTER(u64)]
         L.wva_group_analyze_pairs_loads.argtypes = [vp, i32, abi.f32p, vp, vp]
+        L.wva_solve_capacities.argtypes = [vp, C.POINTER(abi.OptimizerSpec), i32, abi.i64p, abi.i32p, vp, abi.i64p, abi.f32p]
+        L.wva_solve_capacities_counters.argtypes = [vp, C.POINTER(u64)]
+        L.wva_solve_capacities_set_budget.argtypes = [vp, i64]
+        L.wva_group_solve_capacities.argtypes = [vp, C.POINTER(abi.OptimizerSpec), i32, abi.i64p, abi.i32p, vp, abi.i64p, abi.f32p]
         if L.wva_abi_version() != abi.ABI_VERSION:
             raise ImportError("libwva_b200.so ABI version mismatch")
         _lib = L
@@ -153,6 +158,25 @@ def comm_unique_id():
     if rc != abi.OK:
         raise WvaError(rc, lib().wva_last_error(None).decode())
     return bytes(buf.raw)
+
+
+def _capacity_call(fn, h, S, T, capacities, delayed_best_effort, policy, download):
+    """wva_solve_capacities / wva_group_solve_capacities: capacities [n_c, T] -> (chosen_acc [n_c, S], recs [n_c, S] of
+    abi.PAIR_REC_DTYPE, count [n_c, T], cost [n_c, T]), or None when download is False"""
+    cap = np.ascontiguousarray(capacities, dtype=np.int64)
+    if cap.ndim != 2 or cap.shape[1] != T:
+        raise ValueError("capacities must be shaped [n_c, T]")
+    n_c = cap.shape[0]
+    spec = abi.OptimizerSpec(0, 1 if delayed_best_effort else 0, int(policy))
+    if not download:
+        return fn(h, C.byref(spec), n_c, abi.ptr(cap, C.c_int64), None, None, None, None), None
+    acc = np.full((n_c, S), -1, dtype=np.int32)
+    recs = np.zeros((n_c, S), dtype=abi.PAIR_REC_DTYPE)
+    count = np.zeros((n_c, T), dtype=np.int64)
+    cost = np.zeros((n_c, T), dtype=np.float32)
+    rc = fn(h, C.byref(spec), n_c, abi.ptr(cap, C.c_int64), abi.ptr(acc, C.c_int32), recs.ctypes.data, abi.ptr(count, C.c_int64),
+            abi.ptr(cost, C.c_float))
+    return rc, (acc, recs, count, cost)
 
 
 class Context:
@@ -499,6 +523,26 @@ class Context:
         self._ck(lib().wva_solve(self._h, C.byref(spec), abi.ptr(chosen_acc, C.c_int32), C.byref(chosen.c)))
         return chosen_acc, chosen
 
+    def solve_capacities(self, capacities, delayed_best_effort=False, policy=abi.POLICY_NONE, download=True):
+        """Limited solve under each capacity vector of capacities [n_c, T] in one call, on the current pair records, which
+        stay as they are.  Returns (chosen_acc [n_c, S], recs [n_c, S] of abi.PAIR_REC_DTYPE, count [n_c, T], cost [n_c, T]):
+        row j is what set_capacity(capacities[j]), a limited solve, solution_fetch and allocate_by_type give.  None when
+        download is False."""
+        img = self.image
+        rc, out = _capacity_call(lib().wva_solve_capacities, self._h, img.S, img.T, capacities, delayed_best_effort, policy, download)
+        self._ck(rc)
+        return out
+
+    def solve_capacities_counters(self):
+        """counters of the last solve_capacities"""
+        v = (C.c_uint64 * 4)()
+        self._ck(lib().wva_solve_capacities_counters(self._h, v))
+        return dict(chunks=v[0], path=v[1], events=v[2], max_cycles=v[3])
+
+    def solve_capacities_set_budget(self, nbytes):
+        """staging budget of solve_capacities in bytes (0: the default 2^28)"""
+        self._ck(lib().wva_solve_capacities_set_budget(self._h, int(nbytes)))
+
     def solution_fetch(self):
         """The decisions of the last solve (also one made with download=False): (chosen_acc[S], AllocArrays[S])."""
         chosen_acc = np.full(self.image.S, -1, dtype=np.int32)
@@ -663,6 +707,14 @@ class Group:
         chosen = abi.AllocArrays(self.image.S)
         self._ck(lib().wva_group_solve(self._h, C.byref(spec), abi.ptr(chosen_acc, C.c_int32), C.byref(chosen.c)))
         return chosen_acc, chosen
+
+    def solve_capacities(self, capacities, delayed_best_effort=False, policy=abi.POLICY_NONE, download=True):
+        """Context.solve_capacities on every device's gathered rows; device 0 returns the results"""
+        img = self.image
+        rc, out = _capacity_call(lib().wva_group_solve_capacities, self._h, img.S, img.T, capacities, delayed_best_effort, policy,
+                                 download)
+        self._ck(rc)
+        return out
 
     def allocate_by_type(self, download=True):
         if not download:

@@ -207,6 +207,10 @@ struct wva_ctx {
     int greedy_path = 0;        // last limited solve: 1 heap, 2 ranked queue, 3 static-order scan
     uint64_t greedy_stats[4] = {0, 0, 0, 0};
     unsigned long long* greedy_stats_dev = nullptr;
+    // wva_solve_capacities: buffers of its own (greedyBuf holds the last solve's stats), staging budget, counters
+    DevBuf capShared, capSlots, capChunk, capPairs;
+    size_t cap_budget = (size_t)1 << 28;
+    uint64_t cap_counters[4] = {0, 0, 0, 0};
 
     // grid
     DevBuf keys, bestDev, cube, status, counters, gridSlow, gridSlowCount, faultList, faultCount;
@@ -1679,6 +1683,137 @@ int wva_grid_best_blocking(wva_ctx* ctx, float* p_block) {
     return WVA_OK;
 }
 
+}  // extern "C"
+
+// The capacity-independent part of a limited solve, as wva_solve runs it: greedy buffers carved out of `buf`, the
+// per-server candidate order (k_greedy_prepare), the priority buckets and -- on the scan and ranked paths -- the sorted
+// order with its records.  Which path the shape and wva_solve_set_ranked allow lands in p.path (3 scan, 2 ranked, 1 heap).
+struct GreedyPlan {
+    GreedyBufs g; GreedyRank gr; GreedyScan gsc;
+    int* chosenKey;
+    size_t nS, nSA, n2, doneBytes;
+    int path;
+};
+static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
+    const int S = ctx->S, A = ctx->A;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
+    const size_t nS = (size_t)(S ? S : 1);
+    const size_t nSA = nS * A;
+    size_t o_order = take(nSA * 4), o_cand = take(nSA * sizeof(GreedyCand)), o_upr = take(nSA * 8), o_rep = take(nSA * 8), o_ct = take(nSA * 4),
+           o_n = take(nS * 4), o_gs = take(104 * 4), o_gi = take(nS * 4), o_un = take(nS * 4), o_ha = take(nS * 8),
+           o_hb = take(nS * 8), o_hs = take(nS * 4), o_tk = take(nS * sizeof(GreedyTicket)), o_li = take(nS * 4),
+           o_nan = take(8), o_stats = take(32), o_key = take(nS * 4);
+    // ranked queue: states sorted by their fixed key (see k_greedy_solve_ranked)
+    size_t n2 = GREEDY_TILE;
+    while (n2 < nSA) n2 <<= 1;
+    // static-order scan (wva_greedy_scan.cuh): the default; shared memory holds one bit per server
+    const size_t doneBytes = align_up((nS + 31) / 32 * 4, 16);
+    const bool scannable = nSA < (1u << 24) && A <= 32 && doneBytes + 4096 <= (size_t)kGreedySmem && ctx->greedy_ranked >= 2;
+    const bool rankable = !scannable && nSA < (1u << 24) && greedy_bitmap_bytes(nSA, nullptr, nullptr, nullptr) + 4096 <= (size_t)kGreedySmem &&
+                          ctx->greedy_ranked >= 1;
+    size_t o_ka = 0, o_kb = 0, o_ks = 0, o_pos = 0, o_sn = 0, o_rec = 0, o_np = 0, o_ge = 0, o_gb = 0, o_top = 0, o_succ = 0;
+    if (rankable || scannable) {
+        o_ka = take(n2 * 8); o_kb = take(n2 * 4); o_ks = take(n2 * 4); o_pos = take(nSA * 4); o_sn = take(nSA * 4);
+        o_rec = take(n2 * 16); o_np = take(n2 * 8); o_ge = take(n2 * 4); o_gb = take(n2 * 4); o_top = take((n2 + 1) * 4); o_succ = take(nS * 4);
+    }
+    CK(buf.ensure(off));
+    char* b = buf.as<char>();
+    GreedyBufs& g = p.g;
+    g.order = (int*)(b + o_order); g.cand = (GreedyCand*)(b + o_cand); g.upr = (long long*)(b + o_upr); g.rep = (long long*)(b + o_rep);
+    g.ctype = (int*)(b + o_ct); g.nCand = (int*)(b + o_n); g.groupStart = (int*)(b + o_gs); g.groupItems = (int*)(b + o_gi);
+    g.unalloc = (int*)(b + o_un); g.heapA = (unsigned long long*)(b + o_ha); g.heapB = (unsigned long long*)(b + o_hb);
+    g.heapSlot = (unsigned*)(b + o_hs); g.tickets = (GreedyTicket*)(b + o_tk); g.liveIdx = (int*)(b + o_li);
+    g.nanFlag = (int*)(b + o_nan);
+    g.stats = (unsigned long long*)(b + o_stats);
+    g.smemBytes = kGreedySmem;
+    GreedyRank& gr = p.gr;
+    GreedyScan& gsc = p.gsc;
+    gr = GreedyRank{}; gsc = GreedyScan{};
+    if (rankable || scannable) {
+        gr.ka = (unsigned long long*)(b + o_ka); gr.kb = (unsigned*)(b + o_kb); gr.kslot = (unsigned*)(b + o_ks);
+        gr.posOf = (unsigned*)(b + o_pos); gr.snext = (int*)(b + o_sn); gr.rec = (int4*)(b + o_rec); gr.nextPos = (int2*)(b + o_np);
+        gr.gend = (int*)(b + o_ge); gr.gbeg = (int*)(b + o_gb); gr.top = (int*)(b + o_top); gr.succ = (int*)(b + o_succ); gr.n2 = (unsigned)n2;
+        // the scan path lays its arrays over the ranked queue's
+        gsc.ka = gr.ka; gsc.kb = gr.kb; gsc.kslot = gr.kslot; gsc.posOf = gr.posOf; gsc.runHead = (unsigned char*)(b + o_sn);
+        gsc.ev = gr.rec; gsc.push = gr.nextPos; gsc.gbeg = gr.gbeg; gsc.stackTop = gr.top; gsc.stackBuf = gr.gend;
+        gsc.nEv = g.nanFlag; gsc.n2 = (unsigned)n2;
+    }
+    if (!ctx->greedy_attr) {
+        CK(cudaFuncSetAttribute(k_greedy_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
+        CK(cudaFuncSetAttribute(k_greedy_solve_ranked, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
+        CK(cudaFuncSetAttribute(k_greedy_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
+        ctx->greedy_attr = true;
+    }
+    int* chosenKey = (int*)(b + o_key);
+    p.chosenKey = chosenKey;
+    CK(cudaMemsetAsync(g.groupStart, 0, 104 * 4, ctx->stream));
+    CK(cudaMemsetAsync(g.nanFlag, 0, 8, ctx->stream));
+    CK(cudaMemsetAsync(g.stats, 0, 32, ctx->stream));
+    CK(cudaMemsetAsync(chosenKey, 0xff, nS * 4, ctx->stream));
+    if (S > 0) {
+        k_greedy_prepare<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, ctx->pairs, ctx->feasible, g);
+        LAUNCH_CHECK();
+        k_greedy_bucket_count<<<(S + 255) / 256, 256, 0, ctx->stream>>>(ctx->dsys, g);
+        LAUNCH_CHECK();
+        if (rankable || scannable) {
+            const unsigned nb = (unsigned)((n2 + 255) / 256), nt = (unsigned)(n2 / GREEDY_TILE);
+            if (scannable) k_greedy_scan_keys<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gsc);
+            else k_greedy_states<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gr);
+            LAUNCH_CHECK();
+            k_greedy_bitonic_tile<<<nt, 512, 0, ctx->stream>>>(gr, 2u, (unsigned)GREEDY_TILE);
+            LAUNCH_CHECK();
+            for (size_t k = 2 * (size_t)GREEDY_TILE; k <= n2; k <<= 1) {
+                for (size_t j = k >> 1; j >= (size_t)GREEDY_TILE; j >>= 1) {
+                    k_greedy_bitonic_step<<<(unsigned)((n2 / 2 + 255) / 256), 256, 0, ctx->stream>>>(gr, (unsigned)k, (unsigned)j);
+                    LAUNCH_CHECK();
+                }
+                k_greedy_bitonic_tile<<<nt, 512, 0, ctx->stream>>>(gr, (unsigned)k, (unsigned)k);
+                LAUNCH_CHECK();
+            }
+            CK(cudaMemsetAsync(gr.gend, 0, n2 * 4, ctx->stream));
+            CK(cudaMemsetAsync(gr.top, 0, (n2 + 1) * 4, ctx->stream));
+            k_greedy_index<<<nb, 256, 0, ctx->stream>>>(gr);
+            LAUNCH_CHECK();
+            if (scannable) {
+                CK(cudaMemsetAsync(gsc.gbeg, 0xff, n2 * 4, ctx->stream));
+                k_greedy_scan_groups<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, gsc);
+                LAUNCH_CHECK();
+                k_greedy_scan_records<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gsc);
+                LAUNCH_CHECK();
+            } else {
+                k_greedy_tie_groups<<<nb, 256, 0, ctx->stream>>>(gr);
+                LAUNCH_CHECK();
+                k_greedy_records<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gr);
+                LAUNCH_CHECK();
+                k_greedy_tie_init<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gr);
+                LAUNCH_CHECK();
+            }
+        }
+    }
+    p.nS = nS; p.nSA = nSA; p.n2 = n2; p.doneBytes = doneBytes;
+    p.path = scannable ? 3 : rankable ? 2 : 1;
+    return WVA_OK;
+}
+
+// dynamic shared memory of the scan pass: one bit per server, plus the ticket pool of the round-robin policies
+static size_t greedy_scan_smem(const GreedyPlan& p, int policy) {
+    size_t smem = p.doneBytes;
+    const bool tickets = policy == WVA_POLICY_ROUND_ROBIN || policy == WVA_POLICY_PRIORITY_ROUND_ROBIN;
+    if (tickets) smem = std::min((size_t)kGreedySmem, smem + p.nS * (sizeof(GreedyTicket) + 4));
+    return smem;
+}
+// ranked queue: the rank bitmap, plus the ticket pool when a round-robin policy can use it; whatever is not asked for
+// stays L1 for the record loads
+static size_t greedy_ranked_smem(const GreedyPlan& p, int policy) {
+    size_t smem = align_up(greedy_bitmap_bytes(p.nSA, nullptr, nullptr, nullptr), 16);
+    const bool tickets = policy == WVA_POLICY_ROUND_ROBIN || policy == WVA_POLICY_PRIORITY_ROUND_ROBIN;
+    if (tickets) smem = std::min((size_t)kGreedySmem, smem + p.nS * (sizeof(GreedyTicket) + 4));
+    return smem;
+}
+
+extern "C" {
+
 // ---------------------------------------------------------------------------------------------
 int wva_solve(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t* chosen_acc, wva_alloc_soa* chosen) {
     if (!ctx || !spec) return fail(ctx, WVA_EINVAL, "null argument");
@@ -1703,118 +1838,26 @@ int wva_solve(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t* chosen_acc,
         }
         if (!ctx->pairs_complete)
             return fail(ctx, WVA_ESTATE, "limited-capacity solve needs the candidates of every server (wva_comm_init, or gather them and wva_pairs_commit)");
-        // carve greedy buffers
         if (T > 256) return fail(ctx, WVA_EINVAL, "the device greedy solver holds at most 256 accelerator types");
         if ((unsigned long long)(S ? S : 1) * (unsigned long long)A >= (1ull << 31))
             return fail(ctx, WVA_EINVAL, "servers x accelerators must stay below 2^31 for the greedy solver");
-        size_t off = 0;
-        auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-        const size_t nS = (size_t)(S ? S : 1);
-        const size_t nSA = nS * A;
-        size_t o_order = take(nSA * 4), o_cand = take(nSA * sizeof(GreedyCand)), o_upr = take(nSA * 8), o_rep = take(nSA * 8), o_ct = take(nSA * 4),
-               o_n = take(nS * 4), o_gs = take(104 * 4), o_gi = take(nS * 4), o_un = take(nS * 4), o_ha = take(nS * 8),
-               o_hb = take(nS * 8), o_hs = take(nS * 4), o_tk = take(nS * sizeof(GreedyTicket)), o_li = take(nS * 4),
-               o_nan = take(8), o_stats = take(32), o_key = take(nS * 4);
-        // ranked queue: states sorted by their fixed key (see k_greedy_solve_ranked)
-        size_t n2 = GREEDY_TILE;
-        while (n2 < nSA) n2 <<= 1;
-        // static-order scan (wva_greedy_scan.cuh): the default; shared memory holds one bit per server
-        const size_t doneBytes = align_up((nS + 31) / 32 * 4, 16);
-        const bool scannable = nSA < (1u << 24) && A <= 32 && doneBytes + 4096 <= (size_t)kGreedySmem && ctx->greedy_ranked >= 2;
-        const bool rankable = !scannable && nSA < (1u << 24) && greedy_bitmap_bytes(nSA, nullptr, nullptr, nullptr) + 4096 <= (size_t)kGreedySmem &&
-                              ctx->greedy_ranked >= 1;
-        size_t o_ka = 0, o_kb = 0, o_ks = 0, o_pos = 0, o_sn = 0, o_rec = 0, o_np = 0, o_ge = 0, o_gb = 0, o_top = 0, o_succ = 0;
-        if (rankable || scannable) {
-            o_ka = take(n2 * 8); o_kb = take(n2 * 4); o_ks = take(n2 * 4); o_pos = take(nSA * 4); o_sn = take(nSA * 4);
-            o_rec = take(n2 * 16); o_np = take(n2 * 8); o_ge = take(n2 * 4); o_gb = take(n2 * 4); o_top = take((n2 + 1) * 4); o_succ = take(nS * 4);
-        }
-        CK(ctx->greedyBuf.ensure(off));
-        char* b = ctx->greedyBuf.as<char>();
-        GreedyBufs g;
-        g.order = (int*)(b + o_order); g.cand = (GreedyCand*)(b + o_cand); g.upr = (long long*)(b + o_upr); g.rep = (long long*)(b + o_rep);
-        g.ctype = (int*)(b + o_ct); g.nCand = (int*)(b + o_n); g.groupStart = (int*)(b + o_gs); g.groupItems = (int*)(b + o_gi);
-        g.unalloc = (int*)(b + o_un); g.heapA = (unsigned long long*)(b + o_ha); g.heapB = (unsigned long long*)(b + o_hb);
-        g.heapSlot = (unsigned*)(b + o_hs); g.tickets = (GreedyTicket*)(b + o_tk); g.liveIdx = (int*)(b + o_li);
-        g.nanFlag = (int*)(b + o_nan);
-        g.stats = (unsigned long long*)(b + o_stats);
-        g.smemBytes = kGreedySmem;
-        GreedyRank gr{};
-        GreedyScan gsc{};
-        if (rankable || scannable) {
-            gr.ka = (unsigned long long*)(b + o_ka); gr.kb = (unsigned*)(b + o_kb); gr.kslot = (unsigned*)(b + o_ks);
-            gr.posOf = (unsigned*)(b + o_pos); gr.snext = (int*)(b + o_sn); gr.rec = (int4*)(b + o_rec); gr.nextPos = (int2*)(b + o_np);
-            gr.gend = (int*)(b + o_ge); gr.gbeg = (int*)(b + o_gb); gr.top = (int*)(b + o_top); gr.succ = (int*)(b + o_succ); gr.n2 = (unsigned)n2;
-            // the scan path lays its arrays over the ranked queue's
-            gsc.ka = gr.ka; gsc.kb = gr.kb; gsc.kslot = gr.kslot; gsc.posOf = gr.posOf; gsc.runHead = (unsigned char*)(b + o_sn);
-            gsc.ev = gr.rec; gsc.push = gr.nextPos; gsc.gbeg = gr.gbeg; gsc.stackTop = gr.top; gsc.stackBuf = gr.gend;
-            gsc.nEv = g.nanFlag; gsc.n2 = (unsigned)n2;
-        }
-        if (!ctx->greedy_attr) {
-            CK(cudaFuncSetAttribute(k_greedy_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
-            CK(cudaFuncSetAttribute(k_greedy_solve_ranked, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
-            CK(cudaFuncSetAttribute(k_greedy_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
-            ctx->greedy_attr = true;
-        }
-        int* chosenKey = (int*)(b + o_key);
-        CK(cudaMemsetAsync(g.groupStart, 0, 104 * 4, ctx->stream));
-        CK(cudaMemsetAsync(g.nanFlag, 0, 8, ctx->stream));
-        CK(cudaMemsetAsync(g.stats, 0, 32, ctx->stream));
-        CK(cudaMemsetAsync(chosenKey, 0xff, nS * 4, ctx->stream));
+        GreedyPlan gp;
+        int rc = greedy_setup(ctx, ctx->greedyBuf, gp);
+        if (rc != WVA_OK) return rc;
+        GreedyBufs& g = gp.g;
+        GreedyRank& gr = gp.gr;
+        GreedyScan& gsc = gp.gsc;
+        int* chosenKey = gp.chosenKey;
         if (S > 0) {
-            k_greedy_prepare<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, ctx->pairs, ctx->feasible, g);
-            LAUNCH_CHECK();
-            k_greedy_bucket_count<<<(S + 255) / 256, 256, 0, ctx->stream>>>(ctx->dsys, g);
-            LAUNCH_CHECK();
-            if (rankable || scannable) {
-                const unsigned nb = (unsigned)((n2 + 255) / 256), nt = (unsigned)(n2 / GREEDY_TILE);
-                if (scannable) k_greedy_scan_keys<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gsc);
-                else k_greedy_states<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gr);
-                LAUNCH_CHECK();
-                k_greedy_bitonic_tile<<<nt, 512, 0, ctx->stream>>>(gr, 2u, (unsigned)GREEDY_TILE);
-                LAUNCH_CHECK();
-                for (size_t k = 2 * (size_t)GREEDY_TILE; k <= n2; k <<= 1) {
-                    for (size_t j = k >> 1; j >= (size_t)GREEDY_TILE; j >>= 1) {
-                        k_greedy_bitonic_step<<<(unsigned)((n2 / 2 + 255) / 256), 256, 0, ctx->stream>>>(gr, (unsigned)k, (unsigned)j);
-                        LAUNCH_CHECK();
-                    }
-                    k_greedy_bitonic_tile<<<nt, 512, 0, ctx->stream>>>(gr, (unsigned)k, (unsigned)k);
-                    LAUNCH_CHECK();
-                }
-                CK(cudaMemsetAsync(gr.gend, 0, n2 * 4, ctx->stream));
-                CK(cudaMemsetAsync(gr.top, 0, (n2 + 1) * 4, ctx->stream));
-                k_greedy_index<<<nb, 256, 0, ctx->stream>>>(gr);
-                LAUNCH_CHECK();
-                if (scannable) {
-                    CK(cudaMemsetAsync(gsc.gbeg, 0xff, n2 * 4, ctx->stream));
-                    k_greedy_scan_groups<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, gsc);
-                    LAUNCH_CHECK();
-                    k_greedy_scan_records<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gsc);
-                    LAUNCH_CHECK();
-                } else {
-                    k_greedy_tie_groups<<<nb, 256, 0, ctx->stream>>>(gr);
-                    LAUNCH_CHECK();
-                    k_greedy_records<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gr);
-                    LAUNCH_CHECK();
-                    k_greedy_tie_init<<<nb, 256, 0, ctx->stream>>>(ctx->dsys, g, gr);
-                    LAUNCH_CHECK();
-                }
-            }
-            ctx->greedy_path = scannable ? 3 : rankable ? 2 : 1;
+            ctx->greedy_path = gp.path;
             if (ctx->greedy_path == 3) {
-                // shared memory: one bit per server (stopped or not), plus the ticket pool of the round-robin policies
-                size_t smem = doneBytes;
-                const bool tickets = spec->saturation_policy == WVA_POLICY_ROUND_ROBIN || spec->saturation_policy == WVA_POLICY_PRIORITY_ROUND_ROBIN;
-                if (tickets) smem = std::min((size_t)kGreedySmem, smem + nS * (sizeof(GreedyTicket) + 4));
+                const size_t smem = greedy_scan_smem(gp, spec->saturation_policy);
                 g.smemBytes = (int)smem;
                 k_greedy_scan<<<1, 32, smem, ctx->stream>>>(ctx->dsys, ctx->pairs, g, gsc, chosenKey, spec->delayed_best_effort ? 1 : 0,
                                                            spec->saturation_policy);
             }
             else if (ctx->greedy_path == 2) {
-                // shared memory: the rank bitmap, plus the ticket pool when a round-robin policy can
-                // use it; whatever is not asked for stays L1 for the record loads
-                size_t smem = align_up(greedy_bitmap_bytes(nSA, nullptr, nullptr, nullptr), 16);
-                const bool tickets = spec->saturation_policy == WVA_POLICY_ROUND_ROBIN || spec->saturation_policy == WVA_POLICY_PRIORITY_ROUND_ROBIN;
-                if (tickets) smem = std::min((size_t)kGreedySmem, smem + nS * (sizeof(GreedyTicket) + 4));
+                const size_t smem = greedy_ranked_smem(gp, spec->saturation_policy);
                 g.smemBytes = (int)smem;
                 k_greedy_solve_ranked<<<1, 32, smem, ctx->stream>>>(ctx->dsys, ctx->pairs, g, gr, chosenKey,
                                                                    spec->delayed_best_effort ? 1 : 0, spec->saturation_policy);
@@ -1875,6 +1918,191 @@ int wva_solve_greedy_path(const wva_ctx* ctx) { return ctx ? ctx->greedy_path : 
 int wva_solve_stats(wva_ctx* ctx, uint64_t out[4]) {
     if (!ctx || !out) return WVA_EINVAL;
     for (int i = 0; i < 4; ++i) out[i] = ctx->greedy_stats[i];
+    return WVA_OK;
+}
+
+}  // extern "C"
+
+// the argument and state checks of wva_solve_capacities (also run for every member of a group before any device runs)
+static int solve_capacities_check(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n_c, const int64_t* capacity) {
+    if (!spec) return fail(ctx, WVA_EINVAL, "null argument");
+    if (spec->unlimited) return fail(ctx, WVA_EINVAL, "unlimited decisions do not depend on capacities: use wva_solve");
+    if (n_c < 1 || n_c > WVA_SOLVE_MAX_CAPACITIES || !capacity)
+        return fail(ctx, WVA_EINVAL, "capacity list: 1 <= n_c <= 8192 vectors of T counts required");
+    if (!ctx->pairs_valid)
+        return fail(ctx, WVA_ESTATE, "wva_solve_capacities needs the records of wva_analyze_pairs (a limited wva_solve scales them)");
+    if (ctx->T > 256) return fail(ctx, WVA_EINVAL, "the device greedy solver holds at most 256 accelerator types");
+    if ((unsigned long long)(ctx->S ? ctx->S : 1) * (unsigned long long)ctx->A >= (1ull << 31))
+        return fail(ctx, WVA_EINVAL, "servers x accelerators must stay below 2^31 for the greedy solver");
+    if (!ctx->pairs_complete && !ctx->comm)
+        return fail(ctx, WVA_ESTATE, "limited-capacity solve needs the candidates of every server (wva_comm_init, or gather them and wva_pairs_commit)");
+    return WVA_OK;
+}
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------------------
+// Limited solve over a list of capacity vectors.  The capacity-independent part (candidate order, sorted static order,
+// event records) runs once into buffers of this call; then, per chunk of vectors that fits the staging budget, one warp
+// per vector runs the scan pass (k_greedy_scan_multi) with state of its own, k_greedy_collect_multi builds the chosen
+// records from the resident ones, k_totals_multi sums the types, and the chunk is copied out.  Shapes the scan path does
+// not take (or wva_solve_set_ranked < 2) run the ranked-queue or heap kernel once per vector on a copy of the records.
+int wva_solve_capacities(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n_c, const int64_t* capacity, int32_t* chosen_acc,
+                         wva_pair_rec* chosen, int64_t* type_count, float* type_cost) {
+    if (!ctx) return WVA_EINVAL;
+    int rc = solve_capacities_check(ctx, spec, n_c, capacity);
+    if (rc != WVA_OK) return rc;
+    CK(cudaSetDevice(ctx->device));
+    if (!ctx->pairs_complete) {
+        rc = comm_gather_pairs(ctx);
+        if (rc != WVA_OK) return rc;
+    }
+    const int S = ctx->S, T = ctx->T;
+    const int policy = spec->saturation_policy, dbe = spec->delayed_best_effort ? 1 : 0;
+    GreedyPlan gp;
+    rc = greedy_setup(ctx, ctx->capShared, gp);
+    if (rc != WVA_OK) return rc;
+    const int path = S > 0 ? gp.path : 0;
+    GreedyBufs g = gp.g;
+    const size_t nS = gp.nS, n2 = gp.n2;
+    // scan path: compact slots of the positions in shared groups, and the push records pointing at them
+    unsigned P = 0;
+    int nEv = 0;
+    int* slotDev = nullptr; int2* pushSlot = nullptr; unsigned long long* maxCyc = nullptr;
+    if (path == 3) {
+        const unsigned nb = (unsigned)((n2 + 255) / 256);
+        const size_t o_tot = align_up((size_t)nb * 4, 256), o_slot = o_tot + 256, o_push = align_up(o_slot + n2 * 4, 256);
+        CK(ctx->capSlots.ensure(o_push + n2 * 8));
+        char* b = ctx->capSlots.as<char>();
+        int* blockCnt = (int*)b;
+        int* total = (int*)(b + o_tot);
+        maxCyc = (unsigned long long*)(b + o_tot + 8);
+        slotDev = (int*)(b + o_slot); pushSlot = (int2*)(b + o_push);
+        CK(cudaMemsetAsync(b + o_tot, 0, 16, ctx->stream));
+        k_greedy_group_count<<<nb, 256, 0, ctx->stream>>>(gp.gsc, blockCnt);
+        LAUNCH_CHECK();
+        k_greedy_group_offsets<<<1, 1024, 0, ctx->stream>>>(blockCnt, (int)nb, total);
+        LAUNCH_CHECK();
+        k_greedy_group_slots<<<nb, 256, 0, ctx->stream>>>(gp.gsc, blockCnt, slotDev);
+        LAUNCH_CHECK();
+        k_greedy_group_push<<<nb, 256, 0, ctx->stream>>>(gp.gsc, slotDev, pushSlot);
+        LAUNCH_CHECK();
+        int hv[2] = {0, 0};
+        CK(cudaMemcpyAsync(&hv[0], total, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(&hv[1], gp.gsc.nEv, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        P = (unsigned)hv[0]; nEv = hv[1];
+    }
+    // per-vector scratch and outputs; the round-robin ticket pool goes to HBM only when it does not fit shared memory
+    const size_t smem = path == 3 ? greedy_scan_smem(gp, policy) : 0;
+    const bool ticketsHbm = path == 3 && (policy == WVA_POLICY_ROUND_ROBIN || policy == WVA_POLICY_PRIORITY_ROUND_ROBIN) &&
+                            gp.doneBytes + nS * (sizeof(GreedyTicket) + 4) > (size_t)kGreedySmem;
+    size_t perVec = (size_t)T * 8 + (size_t)S * (4 + sizeof(wva_pair_rec)) + (size_t)T * 12;
+    if (path == 3) perVec += (size_t)S * (4 + 4 + 8 + 8) + (size_t)P * 8 + (ticketsHbm ? (size_t)S * (sizeof(GreedyTicket) + 4) : 0);
+    const int nChunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_c, ctx->cap_budget / perVec));
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
+    const size_t nv1 = (size_t)nChunk, nvS = nv1 * S;
+    const size_t o_cap = take(nv1 * T * 8), o_acc = take(nvS * 4), o_rec = take(nvS * sizeof(wva_pair_rec)), o_cnt = take(nv1 * T * 8),
+                 o_cost = take(nv1 * T * 4);
+    size_t o_key = 0, o_un = 0, o_got = 0, o_cur = 0, o_top = 0, o_buf = 0, o_tk = 0, o_li = 0;
+    if (path == 3) {
+        o_key = take(nvS * 4); o_un = take(nvS * 4); o_got = take(nvS * 8); o_cur = take(nvS * 8); o_top = take(nv1 * P * 4); o_buf = take(nv1 * P * 4);
+        if (ticketsHbm) { o_tk = take(nvS * sizeof(GreedyTicket)); o_li = take(nvS * 4); }
+    }
+    CK(ctx->capChunk.ensure(off));
+    char* cb = ctx->capChunk.as<char>();
+    long long* capDev = (long long*)(cb + o_cap);
+    int* accDev = (int*)(cb + o_acc);
+    wva_pair_rec* recDev = (wva_pair_rec*)(cb + o_rec);
+    long long* cntDev = (long long*)(cb + o_cnt);
+    float* costDev = (float*)(cb + o_cost);
+    // the ranked-queue and heap kernels scale the records they are given: a copy of the three fields they write
+    DevAllocs work = ctx->pairs;
+    if (path == 1 || path == 2) {
+        const size_t nSA = gp.nSA;
+        CK(ctx->capPairs.ensure(align_up(nSA * 8, 256) + 2 * align_up(nSA * 4, 256)));
+        char* pb = ctx->capPairs.as<char>();
+        work.num_replicas = (long long*)pb; work.cost = (float*)(pb + align_up(nSA * 8, 256));
+        work.value = (float*)(pb + align_up(nSA * 8, 256) + align_up(nSA * 4, 256));
+    }
+    if (path == 3 && smem > 48 * 1024) CK(cudaFuncSetAttribute(k_greedy_scan_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    uint64_t chunks = 0;
+    for (int v0 = 0; v0 < n_c; v0 += nChunk) {
+        const int nv = std::min(nChunk, n_c - v0);
+        const size_t n = (size_t)nv * S;
+        if (T > 0) CK(cudaMemcpyAsync(capDev, capacity + (size_t)v0 * T, (size_t)nv * T * 8, cudaMemcpyHostToDevice, ctx->stream));
+        if (path == 3) {
+            GreedyScanVecs v;
+            v.capacity = capDev; v.chosen = (int*)(cb + o_key); v.unalloc = (int*)(cb + o_un);
+            v.tickets = ticketsHbm ? (GreedyTicket*)(cb + o_tk) : nullptr; v.liveIdx = ticketsHbm ? (int*)(cb + o_li) : nullptr;
+            v.got = (long long*)(cb + o_got); v.cur = (long long*)(cb + o_cur);
+            v.stackTop = (int*)(cb + o_top); v.stackBuf = (int*)(cb + o_buf); v.P = P; v.maxCycles = maxCyc;
+            CK(cudaMemsetAsync(v.chosen, 0xff, n * 4, ctx->stream));
+            CK(cudaMemsetAsync(v.got, 0, n * 8, ctx->stream));
+            if (P > 0) CK(cudaMemsetAsync(v.stackTop, 0, (size_t)nv * P * 4, ctx->stream));
+            g.smemBytes = (int)smem;
+            k_greedy_scan_multi<<<nv, 32, smem, ctx->stream>>>(ctx->dsys, g, gp.gsc, slotDev, pushSlot, v, dbe, policy);
+            LAUNCH_CHECK();
+            k_greedy_collect_multi<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(ctx->dsys, ctx->pairs, g.order, v.chosen, v.got, v.cur, n,
+                                                                                      accDev, recDev);
+            LAUNCH_CHECK();
+        } else if (path != 0) {
+            const size_t nSA = gp.nSA;
+            for (int j = 0; j < nv; ++j) {
+                DevSystem sys = ctx->dsys;
+                sys.type_capacity = capDev + (size_t)j * T;
+                CK(cudaMemcpyAsync(work.num_replicas, ctx->pairs.num_replicas, nSA * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+                CK(cudaMemcpyAsync(work.cost, ctx->pairs.cost, nSA * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+                CK(cudaMemcpyAsync(work.value, ctx->pairs.value, nSA * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+                // per-solve state: the chosen slots, the priority buckets (k_greedy_solve turns them into offsets in place),
+                // and the ranked queue's tie-group records and counters
+                CK(cudaMemsetAsync(gp.chosenKey, 0xff, nS * 4, ctx->stream));
+                CK(cudaMemsetAsync(g.groupStart, 0, 104 * 4, ctx->stream));
+                k_greedy_bucket_count<<<(S + 255) / 256, 256, 0, ctx->stream>>>(sys, g);
+                LAUNCH_CHECK();
+                if (path == 2) {
+                    const unsigned nb = (unsigned)((n2 + 255) / 256);
+                    CK(cudaMemsetAsync(gp.gr.top, 0, (n2 + 1) * 4, ctx->stream));
+                    k_greedy_records<<<nb, 256, 0, ctx->stream>>>(sys, g, gp.gr);
+                    LAUNCH_CHECK();
+                    k_greedy_tie_init<<<nb, 256, 0, ctx->stream>>>(sys, g, gp.gr);
+                    LAUNCH_CHECK();
+                    const size_t rsmem = greedy_ranked_smem(gp, policy);
+                    GreedyBufs gj = g; gj.smemBytes = (int)rsmem;
+                    k_greedy_solve_ranked<<<1, 32, rsmem, ctx->stream>>>(sys, work, gj, gp.gr, gp.chosenKey, dbe, policy);
+                } else
+                    k_greedy_solve<<<1, 32, kGreedySmem, ctx->stream>>>(sys, work, g, gp.chosenKey, dbe, policy);
+                LAUNCH_CHECK();
+                k_greedy_collect_multi<<<(S + 127) / 128, 128, 0, ctx->stream>>>(sys, work, g.order, gp.chosenKey, nullptr, nullptr, (size_t)S,
+                                                                              accDev + (size_t)j * S, recDev + (size_t)j * S);
+                LAUNCH_CHECK();
+            }
+        }
+        if (T > 0) {
+            k_totals_multi<<<dim3((unsigned)T, (unsigned)nv), 1024, 0, ctx->stream>>>(ctx->dsys, accDev, recDev, cntDev, costDev);
+            LAUNCH_CHECK();
+        }
+        if (chosen_acc && n) CK(cudaMemcpyAsync(chosen_acc + (size_t)v0 * S, accDev, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        if (chosen && n) CK(cudaMemcpyAsync(chosen + (size_t)v0 * S, recDev, n * sizeof(wva_pair_rec), cudaMemcpyDeviceToHost, ctx->stream));
+        if (type_count && T) CK(cudaMemcpyAsync(type_count + (size_t)v0 * T, cntDev, (size_t)nv * T * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        if (type_cost && T) CK(cudaMemcpyAsync(type_cost + (size_t)v0 * T, costDev, (size_t)nv * T * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));       // the next chunk reuses the chunk's buffers
+        ++chunks;
+    }
+    unsigned long long cyc = 0;
+    if (maxCyc) CK(cudaMemcpy(&cyc, maxCyc, 8, cudaMemcpyDeviceToHost));
+    ctx->cap_counters[0] = chunks; ctx->cap_counters[1] = (uint64_t)path; ctx->cap_counters[2] = (uint64_t)nEv; ctx->cap_counters[3] = cyc;
+    return WVA_OK;
+}
+int wva_solve_capacities_counters(const wva_ctx* ctx, uint64_t out[4]) {
+    if (!ctx || !out) return WVA_EINVAL;
+    for (int k = 0; k < 4; ++k) out[k] = ctx->cap_counters[k];
+    return WVA_OK;
+}
+int wva_solve_capacities_set_budget(wva_ctx* ctx, int64_t bytes) {
+    if (!ctx || bytes < 0) return WVA_EINVAL;
+    ctx->cap_budget = bytes == 0 ? (size_t)1 << 28 : (size_t)bytes;
     return WVA_OK;
 }
 
@@ -2285,6 +2513,22 @@ int wva_group_solve(wva_group* g, const wva_optimizer_spec* spec, int32_t* chose
     return g->each([&](int i, wva_ctx* c) {
         const bool mine = spec->unlimited || i == 0;
         return wva_solve(c, spec, mine ? chosen_acc : nullptr, mine ? chosen : nullptr);
+    });
+}
+
+int wva_group_solve_capacities(wva_group* g, const wva_optimizer_spec* spec, int32_t n_c, const int64_t* capacity, int32_t* chosen_acc,
+                               wva_pair_rec* chosen, int64_t* type_count, float* type_cost) {
+    if (!g) return WVA_EINVAL;
+    // every member is checked before any device runs: a member that fails must not leave the others inside the pair all-gather
+    for (wva_ctx* c : g->ctxs) {
+        const int rc = solve_capacities_check(c, spec, n_c, capacity);
+        if (rc != WVA_OK) { g->err = "device " + std::to_string(c->device) + ": " + wva_last_error(c); return rc; }
+    }
+    // every member runs the solves on its gathered rows; they agree, and member 0 returns the results
+    return g->each([&](int i, wva_ctx* c) {
+        const bool mine = i == 0;
+        return wva_solve_capacities(c, spec, n_c, capacity, mine ? chosen_acc : nullptr, mine ? chosen : nullptr,
+                                    mine ? type_count : nullptr, mine ? type_cost : nullptr);
     });
 }
 

@@ -2603,12 +2603,25 @@ __device__ __forceinline__ void greedy_scale(GreedyCtx& c, int s, int slot, long
     c.chosen[s] = slot;
 }
 
+// The same step for a solve that must leave the candidate records as they are (wva_solve_capacities): the scaling is
+// recorded per server -- k_greedy_collect_multi applies it to a copy of the record
+struct GreedyCtxMulti : GreedyCtx {
+    long long* got;            // [S] replicas handed out, 0 where the server was not scaled
+    long long* cur;            // [S] replicas the candidate wanted
+};
+__device__ __forceinline__ void greedy_scale(GreedyCtxMulti& c, int s, int slot, long long got, long long cur) {
+    c.got[s] = got;
+    c.cur[s] = cur;
+    c.chosen[s] = slot;
+}
+
 // allocateMaximally, greedy.go:194-223, 32 servers of the list at a time: lane l owns server l and a cursor over its
 // candidates.  Inside this function `available` only shrinks (a server takes maxReplicas * upr <= available), so a
 // candidate without room for one replica now never gets it later and the cursor only moves forward.  The lanes that found
 // a candidate are then served in list order; after each one the lanes waiting on the same accelerator type look again
 // (same candidate first).  The records of the 32 winners are scaled together at the end (greedy.go:208-212).
-__device__ void greedy_allocate_maximally(GreedyCtx& c, const int* list, int n) {
+template <class Ctx>
+__device__ void greedy_allocate_maximally(Ctx& c, const int* list, int n) {
     const unsigned FULL = 0xffffffffu;
     const int A = c.sys.A;
     for (int i0 = 0; i0 < n; i0 += 32) {
@@ -2656,7 +2669,8 @@ __device__ void greedy_allocate_maximally(GreedyCtx& c, const int* list, int n) 
 }
 
 // allocateEqually, greedy.go:239-316
-__device__ void greedy_allocate_equally(GreedyCtx& c, const int* list, int n) {
+template <class Ctx>
+__device__ void greedy_allocate_equally(Ctx& c, const int* list, int n) {
     const int A = c.sys.A;
     GreedyTicket* tk; int* liveIdx;
     if ((size_t)n * (sizeof(GreedyTicket) + 4) <= (size_t)c.g.smemBytes) {
@@ -2746,7 +2760,8 @@ __device__ void greedy_allocate_equally(GreedyCtx& c, const int* list, int n) {
 }
 
 // bestEffort, greedy.go:169-190 (list is grouped by priority already)
-__device__ void greedy_best_effort(GreedyCtx& c, const int* list, int n, int policy) {
+template <class Ctx>
+__device__ void greedy_best_effort(Ctx& c, const int* list, int n, int policy) {
     if (policy == WVA_POLICY_PRIORITY_EXHAUSTIVE) greedy_allocate_maximally(c, list, n);
     else if (policy == WVA_POLICY_ROUND_ROBIN) greedy_allocate_equally(c, list, n);
     else if (policy == WVA_POLICY_PRIORITY_ROUND_ROBIN) {

@@ -1,0 +1,23 @@
+/* The capacity-list solve through plain C99, the way a cgo preamble compiles the header: the declarations are valid C,
+ * the symbols link, and every entry point rejects a missing context without touching a device. */
+#include <stdint.h>
+#include <stdio.h>
+
+#include "wva_b200.h"
+
+int main(void) {
+    int (*solve)(wva_ctx*, const wva_optimizer_spec*, int32_t, const int64_t*, int32_t*, wva_pair_rec*, int64_t*, float*) =
+        wva_solve_capacities;
+    int (*group)(wva_group*, const wva_optimizer_spec*, int32_t, const int64_t*, int32_t*, wva_pair_rec*, int64_t*, float*) =
+        wva_group_solve_capacities;
+    wva_optimizer_spec spec = {0, 0, WVA_POLICY_NONE};
+    int64_t cap[2] = {1, 2};
+    uint64_t counters[4];
+    if (WVA_SOLVE_MAX_CAPACITIES != 8192) { printf("bad limit\n"); return 1; }
+    if (solve(NULL, &spec, 1, cap, NULL, NULL, NULL, NULL) != WVA_EINVAL) { printf("solve(NULL)\n"); return 1; }
+    if (group(NULL, &spec, 1, cap, NULL, NULL, NULL, NULL) != WVA_EINVAL) { printf("group(NULL)\n"); return 1; }
+    if (wva_solve_capacities_counters(NULL, counters) != WVA_EINVAL) { printf("counters(NULL)\n"); return 1; }
+    if (wva_solve_capacities_set_budget(NULL, 0) != WVA_EINVAL) { printf("set_budget(NULL)\n"); return 1; }
+    printf("solve_capacities c99: ok\n");
+    return 0;
+}

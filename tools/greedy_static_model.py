@@ -73,7 +73,8 @@ def static_order(servers):
     return ev
 
 
-def static_allocate(servers, avail):
+def static_allocate(servers, avail, pushes=None):
+    """pushes, when a list: receives (group key, run-head event index) of every run pushed onto a shared group's stack"""
     avail = list(avail)
     ev = static_order(servers)
     n = len(ev)
@@ -119,6 +120,8 @@ def static_allocate(servers, avail):
         g = ev[h][0]
         if multi[g]:
             stacks.setdefault(g, []).append(h)
+            if pushes is not None:
+                pushes.append((g, h))
 
     # which groups hold more than one server
     multi = {}
