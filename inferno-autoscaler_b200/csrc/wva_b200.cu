@@ -1796,20 +1796,44 @@ static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
     return WVA_OK;
 }
 
-// dynamic shared memory of the scan pass: one bit per server, plus the ticket pool of the round-robin policies
-static size_t greedy_scan_smem(const GreedyPlan& p, int policy) {
-    size_t smem = p.doneBytes;
+// the ticket pool of the round-robin policies: a GreedyTicket and an index per server (none for the other policies)
+static size_t greedy_ticket_bytes(const GreedyPlan& p, int policy) {
     const bool tickets = policy == WVA_POLICY_ROUND_ROBIN || policy == WVA_POLICY_PRIORITY_ROUND_ROBIN;
-    if (tickets) smem = std::min((size_t)kGreedySmem, smem + p.nS * (sizeof(GreedyTicket) + 4));
-    return smem;
+    return tickets ? p.nS * (sizeof(GreedyTicket) + 4) : 0;
+}
+// The scan pass keeps the whole ticket pool in shared memory after its stopped bits (one bit per server) when both fit;
+// otherwise it takes all the shared memory there is and the lists that do not fit it use a pool in HBM.
+static bool greedy_scan_tickets_fit(const GreedyPlan& p, int policy) {
+    return p.doneBytes + greedy_ticket_bytes(p, policy) <= (size_t)kGreedySmem;
+}
+// dynamic shared memory of the scan pass
+static size_t greedy_scan_smem(const GreedyPlan& p, int policy) {
+    return greedy_scan_tickets_fit(p, policy) ? p.doneBytes + greedy_ticket_bytes(p, policy) : (size_t)kGreedySmem;
 }
 // ranked queue: the rank bitmap, plus the ticket pool when a round-robin policy can use it; whatever is not asked for
 // stays L1 for the record loads
 static size_t greedy_ranked_smem(const GreedyPlan& p, int policy) {
-    size_t smem = align_up(greedy_bitmap_bytes(p.nSA, nullptr, nullptr, nullptr), 16);
-    const bool tickets = policy == WVA_POLICY_ROUND_ROBIN || policy == WVA_POLICY_PRIORITY_ROUND_ROBIN;
-    if (tickets) smem = std::min((size_t)kGreedySmem, smem + p.nS * (sizeof(GreedyTicket) + 4));
-    return smem;
+    const size_t smem = align_up(greedy_bitmap_bytes(p.nSA, nullptr, nullptr, nullptr), 16);
+    return std::min((size_t)kGreedySmem, smem + greedy_ticket_bytes(p, policy));
+}
+
+// The sequential kernel of the plan's path, with its dynamic shared memory, under sys's capacities.  Best effort scales
+// the chosen records of `pairs` in place; the chosen slots land in p.chosenKey and the scan path's counters in p.g.stats.
+static int greedy_launch(wva_ctx* ctx, const GreedyPlan& p, const DevSystem& sys, const DevAllocs& pairs, int delayedBestEffort,
+                         int policy) {
+    GreedyBufs g = p.g;
+    if (p.path == 3) {
+        const size_t smem = greedy_scan_smem(p, policy);
+        g.smemBytes = (int)smem;
+        k_greedy_scan<<<1, 32, smem, ctx->stream>>>(sys, pairs, g, p.gsc, p.chosenKey, delayedBestEffort, policy);
+    } else if (p.path == 2) {
+        const size_t smem = greedy_ranked_smem(p, policy);
+        g.smemBytes = (int)smem;
+        k_greedy_solve_ranked<<<1, 32, smem, ctx->stream>>>(sys, pairs, g, p.gr, p.chosenKey, delayedBestEffort, policy);
+    } else
+        k_greedy_solve<<<1, 32, kGreedySmem, ctx->stream>>>(sys, pairs, g, p.chosenKey, delayedBestEffort, policy);
+    LAUNCH_CHECK();
+    return WVA_OK;
 }
 
 extern "C" {
@@ -1844,30 +1868,13 @@ int wva_solve(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t* chosen_acc,
         GreedyPlan gp;
         int rc = greedy_setup(ctx, ctx->greedyBuf, gp);
         if (rc != WVA_OK) return rc;
-        GreedyBufs& g = gp.g;
-        GreedyRank& gr = gp.gr;
-        GreedyScan& gsc = gp.gsc;
-        int* chosenKey = gp.chosenKey;
         if (S > 0) {
             ctx->greedy_path = gp.path;
-            if (ctx->greedy_path == 3) {
-                const size_t smem = greedy_scan_smem(gp, spec->saturation_policy);
-                g.smemBytes = (int)smem;
-                k_greedy_scan<<<1, 32, smem, ctx->stream>>>(ctx->dsys, ctx->pairs, g, gsc, chosenKey, spec->delayed_best_effort ? 1 : 0,
-                                                           spec->saturation_policy);
-            }
-            else if (ctx->greedy_path == 2) {
-                const size_t smem = greedy_ranked_smem(gp, spec->saturation_policy);
-                g.smemBytes = (int)smem;
-                k_greedy_solve_ranked<<<1, 32, smem, ctx->stream>>>(ctx->dsys, ctx->pairs, g, gr, chosenKey,
-                                                                   spec->delayed_best_effort ? 1 : 0, spec->saturation_policy);
-            }
-            else
-                k_greedy_solve<<<1, 32, kGreedySmem, ctx->stream>>>(ctx->dsys, ctx->pairs, g, chosenKey, spec->delayed_best_effort ? 1 : 0,
-                                                                   spec->saturation_policy);
-            LAUNCH_CHECK();
-            ctx->greedy_stats_dev = g.stats;
-            k_greedy_collect<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, ctx->pairs, g.order, chosenKey, ctx->chosen_acc, ctx->chosen);
+            rc = greedy_launch(ctx, gp, ctx->dsys, ctx->pairs, spec->delayed_best_effort ? 1 : 0, spec->saturation_policy);
+            if (rc != WVA_OK) return rc;
+            ctx->greedy_stats_dev = gp.g.stats;
+            k_greedy_collect<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, ctx->pairs, gp.g.order, gp.chosenKey, ctx->chosen_acc,
+                                                                       ctx->chosen);
             LAUNCH_CHECK();
         }
         // best-effort scaling mutated the candidate records in place (greedy.go:208-212): the
@@ -1995,10 +2002,9 @@ int wva_solve_capacities(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n
     }
     // per-vector scratch and outputs; the round-robin ticket pool goes to HBM only when it does not fit shared memory
     const size_t smem = path == 3 ? greedy_scan_smem(gp, policy) : 0;
-    const bool ticketsHbm = path == 3 && (policy == WVA_POLICY_ROUND_ROBIN || policy == WVA_POLICY_PRIORITY_ROUND_ROBIN) &&
-                            gp.doneBytes + nS * (sizeof(GreedyTicket) + 4) > (size_t)kGreedySmem;
+    const bool ticketsHbm = path == 3 && !greedy_scan_tickets_fit(gp, policy);
     size_t perVec = (size_t)T * 8 + (size_t)S * (4 + sizeof(wva_pair_rec)) + (size_t)T * 12;
-    if (path == 3) perVec += (size_t)S * (4 + 4 + 8 + 8) + (size_t)P * 8 + (ticketsHbm ? (size_t)S * (sizeof(GreedyTicket) + 4) : 0);
+    if (path == 3) perVec += (size_t)S * (4 + 4 + 8 + 8) + (size_t)P * 8 + (ticketsHbm ? greedy_ticket_bytes(gp, policy) : 0);
     const int nChunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_c, ctx->cap_budget / perVec));
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
@@ -2068,12 +2074,9 @@ int wva_solve_capacities(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n
                     LAUNCH_CHECK();
                     k_greedy_tie_init<<<nb, 256, 0, ctx->stream>>>(sys, g, gp.gr);
                     LAUNCH_CHECK();
-                    const size_t rsmem = greedy_ranked_smem(gp, policy);
-                    GreedyBufs gj = g; gj.smemBytes = (int)rsmem;
-                    k_greedy_solve_ranked<<<1, 32, rsmem, ctx->stream>>>(sys, work, gj, gp.gr, gp.chosenKey, dbe, policy);
-                } else
-                    k_greedy_solve<<<1, 32, kGreedySmem, ctx->stream>>>(sys, work, g, gp.chosenKey, dbe, policy);
-                LAUNCH_CHECK();
+                }
+                rc = greedy_launch(ctx, gp, sys, work, dbe, policy);
+                if (rc != WVA_OK) return rc;
                 k_greedy_collect_multi<<<(S + 127) / 128, 128, 0, ctx->stream>>>(sys, work, g.order, gp.chosenKey, nullptr, nullptr, (size_t)S,
                                                                               accDev + (size_t)j * S, recDev + (size_t)j * S);
                 LAUNCH_CHECK();

@@ -198,9 +198,8 @@ __device__ __forceinline__ void greedy_scan_batch(GreedyCtx& c, const GreedyScan
     __syncwarp();
 }
 
-// The pass of k_greedy_scan (below) for a context whose state is its own, as k_greedy_scan_multi runs it per vector.
-// k_greedy_scan keeps its own copy of this body, so that wva_solve's kernel compiles exactly as before.  c holds the
-// context without its pool; `capacity` the T starting capacities.
+// The pass over the static order, one warp: k_greedy_scan runs it once on wva_solve's state, k_greedy_scan_multi once per
+// capacity vector on state of the vector's own.  c holds the context without its pool; `capacity` the T starting capacities.
 // groupSlot maps the position where a shared group starts to the index of its stack in gs.stackTop / gs.stackBuf, and
 // gs.n2 bounds gs.stackBuf.  st = the four words of wva_solve_stats.
 template <class Ctx, class GroupSlot>
@@ -303,111 +302,16 @@ __device__ __forceinline__ void greedy_scan_pass(Ctx& c, const GreedyScan& gs, c
     st[0] = (unsigned long long)nEv + (nGroups << 32); st[1] = nBatches + (nPopped << 32); st[2] = cycScan; st[3] = cycBest;
 }
 
-
-// greedy_scan_pass above is a copy of this kernel's pass for k_greedy_scan_multi: a change to one is a change to both
-// (tests/test_solve_capacities_cpu.py checks that they differ only in the context setup, the capacity source, the group
-// slot and the stats write).
 __global__ void __launch_bounds__(32) k_greedy_scan(DevSystem sys, DevAllocs pairs, GreedyBufs g, GreedyScan gs, int* chosen,
                                                       int delayedBestEffort, int policy) {
     extern __shared__ __align__(16) unsigned char greedy_pool[];
     __shared__ long long avail[256];
     __shared__ long long usum[256];
     if (blockIdx.x != 0) return;
-    const unsigned FULL = 0xffffffffu;
-    const int lane = threadIdx.x;
-    const unsigned A = (unsigned)sys.A;
-    unsigned* doneBits = reinterpret_cast<unsigned*>(greedy_pool);
-    const size_t doneWords = ((size_t)sys.S + 31) / 32;
-    const size_t doneBytes = (doneWords * 4 + 15) & ~(size_t)15;
-    GreedyCtx c; c.sys = sys; c.pairs = pairs; c.g = g; c.chosen = chosen; c.avail = avail; c.usum = usum; c.lane = lane;
-    c.pool = greedy_pool + doneBytes;
-    c.g.smemBytes = g.smemBytes - (int)doneBytes;
-    for (int t = lane; t < sys.T; t += 32) avail[t] = sys.type_capacity[t];
-    for (size_t i = lane; i < doneWords; i += 32) doneBits[i] = 0;
-    __syncwarp();
-    const int nEv = *gs.nEv;
-    // runs popped from a stack: 32 / W at a time, W lanes each (a run has at most A events)
-    const int W = A <= 8 ? 8 : (A <= 16 ? 16 : 32);
-    const int perPop = 32 / W;
-    const unsigned lt = (1u << lane) - 1u;
-    int curPr = -1, nUn = 0;
-    unsigned long long cycScan = 0, cycBest = 0, nBatches = 0, nPopped = 0, nGroups = 0;
-    const int4 none = make_int4(0, 0, 0, 0);
-    int4 nextRec = lane < nEv ? gs.ev[lane] : none;
-    int2 nextPush = lane < nEv ? gs.push[lane] : make_int2(0, 0);
-    GreedyPend pd; pd.old = 0; pd.leader = 0; pd.rank = 0; pd.h = 0; pd.g0 = 0; pd.on = false;
-    long long t0 = clock64();
-    for (int base = 0; base < nEv; base += 32) {
-        const int4 rec = nextRec;
-        const int2 pushInfo = nextPush;
-        if (base + 32 + lane < nEv) { nextRec = gs.ev[base + 32 + lane]; nextPush = gs.push[base + 32 + lane]; }
-        const bool valid = base + lane < nEv;
-        const int flags = rec.z, s = rec.w;
-        const long long count = (long long)(((unsigned long long)(unsigned)rec.y << 32) | (unsigned)rec.x);
-        const int pr = (flags >> 18) & 0x7f;
-        const unsigned mValid = __ballot_sync(FULL, valid);
-        const unsigned mG = __ballot_sync(FULL, valid && (flags & GREEDY_GSTART));
-        // where the block has to be cut: a shared group starts (its stack goes first) or the priority changes
-        const int prPrev = __shfl_up_sync(FULL, pr, 1);
-        const unsigned mCut = __ballot_sync(FULL, valid && ((flags & GREEDY_GSTART) || (lane > 0 && pr != prPrev)));
-        int lo = 0;
-        while (lo < 32 && (mValid >> lo)) {
-            // a new priority: bestEffort for the group that ends here (greedy.go:96-103)
-            const int prLo = __shfl_sync(FULL, pr, lo);
-            if (prLo != curPr) {
-                if (curPr >= 0 && !delayedBestEffort) {
-                    const long long t1 = clock64();
-                    greedy_best_effort(c, g.unalloc, nUn, policy);
-                    nUn = 0;
-                    const long long t2 = clock64();
-                    cycScan += (unsigned long long)(t1 - t0); cycBest += (unsigned long long)(t2 - t1); t0 = t2;
-                }
-                curPr = prLo;
-            }
-            // a shared group starts at lo: the runs inserted so far go first, the most recent one on top
-            if ((mG >> lo) & 1u) {
-                const int g0 = base + lo;
-                greedy_scan_flush(gs, pd);                         // pushes still in flight may belong to this group
-                // the count and the first 32 entries travel together (one exposed latency), the runs' records are the second
-                int top = *((volatile int*)gs.stackTop + g0);
-                const int hMine = (unsigned)(g0 + lane) < gs.n2 ? ((volatile int*)gs.stackBuf)[g0 + lane] : -1;
-                if (top > 0) ++nGroups;
-                while (top > 0) {
-                    const int q = lane / W, off = lane - q * W;
-                    const int k = top < perPop ? top : perPop;
-                    const int idx = top - 1 - q;                  // run q of this round: the stack's entry idx
-                    const bool mine = q < k;
-                    const int hv = __shfl_sync(FULL, hMine, mine && idx < 32 ? idx : 0);
-                    int h = -1;
-                    if (mine) h = idx < 32 ? hv : ((volatile int*)gs.stackBuf)[g0 + idx];
-                    int4 r2 = none; int2 p2 = make_int2(0, 0); bool v2 = false;
-                    if (h >= 0 && h + off < nEv) { r2 = gs.ev[h + off]; p2 = gs.push[h + off]; v2 = true; }
-                    const int s2 = v2 ? r2.w : -1;
-                    const int sHead = __shfl_sync(FULL, s2, q * W);
-                    bool ok = v2 && s2 == sHead && (off == 0 || !(r2.z & GREEDY_RUNHEAD));
-                    const unsigned seg = (W == 32 ? FULL : ((1u << W) - 1u) << (q * W));
-                    const unsigned bad = __ballot_sync(FULL, !ok);
-                    ok = ok && !(bad & seg & lt);                  // the run is the contiguous stretch after its head
-                    const int s2c = s2 < 0 ? 0 : s2;
-                    const bool alive2 = ok && !((doneBits[s2c >> 5] >> (s2c & 31)) & 1u);
-                    const long long count2 = (long long)(((unsigned long long)(unsigned)r2.y << 32) | (unsigned)r2.x);
-                    greedy_scan_batch(c, gs, doneBits, alive2, count2, r2.z, s2c, p2, pd, nUn);
-                    top -= k; nPopped += (unsigned long long)k;
-                }
-            }
-            // up to the next shared group or priority
-            const unsigned stop = mCut & ~((2u << lo) - 1u);
-            const int hi = stop ? __ffs(stop) - 1 : 32;
-            const bool alive = valid && lane >= lo && lane < hi && !(flags & GREEDY_STACKED) && !((doneBits[s >> 5] >> (s & 31)) & 1u);
-            greedy_scan_batch(c, gs, doneBits, alive, count, flags, s, pushInfo, pd, nUn);
-            ++nBatches;
-            lo = hi;
-        }
-    }
-    const long long t1 = clock64();
-    greedy_best_effort(c, g.unalloc, nUn, policy);
-    cycScan += (unsigned long long)(t1 - t0); cycBest += (unsigned long long)(clock64() - t1);
-    if (lane == 0) { g.stats[0] = (unsigned long long)nEv + (nGroups << 32); g.stats[1] = nBatches + (nPopped << 32); g.stats[2] = cycScan; g.stats[3] = cycBest; }
+    GreedyCtx c; c.sys = sys; c.pairs = pairs; c.g = g; c.chosen = chosen; c.avail = avail; c.usum = usum; c.lane = threadIdx.x;
+    unsigned long long st[4];
+    greedy_scan_pass(c, gs, sys.type_capacity, greedy_pool, delayedBestEffort, policy, [](int g0) { return g0; }, st);
+    if (threadIdx.x == 0) { g.stats[0] = st[0]; g.stats[1] = st[1]; g.stats[2] = st[2]; g.stats[3] = st[3]; }
 }
 
 // ---- many capacity vectors over one static order (wva_solve_capacities) --------------------------------------------
@@ -520,49 +424,20 @@ __global__ void k_greedy_collect_multi(DevSystem sys, DevAllocs pairs, const int
     chosen[i] = to_pair_rec(r, key >= 0);
 }
 
+// the chosen records of one vector of wva_solve_capacities: chosen_acc[s] >= 0 marks a chosen server
+struct TotalsPairRec {
+    const int* __restrict__ chosen_acc; const wva_pair_rec* __restrict__ rec;
+    __device__ bool chosen(int s) const { return chosen_acc[s] >= 0; }
+    __device__ int acc(int s) const { return rec[s].acc; }
+    __device__ long long replicas(int s) const { return rec[s].num_replicas; }
+    __device__ float cost(int s) const { return rec[s].cost; }
+};
+
 // k_totals over every server for each vector of a chunk: block (t, j) sums type t of vector j in k_totals' order
 __global__ void __launch_bounds__(1024) k_totals_multi(DevSystem sys, const int* __restrict__ chosen_acc, const wva_pair_rec* __restrict__ chosen,
                                                        long long* __restrict__ count, float* __restrict__ cost) {
-    __shared__ float vals[1024];
-    __shared__ long long part[32];
-    const int t = blockIdx.x;
     const size_t j = blockIdx.y;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int ns = sys.S;
-    const int* acc = chosen_acc + j * ns;
-    const wva_pair_rec* rec = chosen + j * ns;
-    long long c = 0; float k = 0.0f;
-    for (int base = 0; base < ns; base += 1024) {
-        const int s = base + tid;
-        float v = 0.0f;
-        if (s < ns && acc[s] >= 0) {
-            const int gi = rec[s].acc;
-            const int m = sys.srv_model[s];
-            if (gi >= 0 && m >= 0 && sys.acc_type[gi] == t) {
-                c += go_muli(go_muli(rec[s].num_replicas, num_instances(sys, m, gi)), (long long)sys.acc_multiplicity[gi]);
-                v = rec[s].cost;
-            }
-        }
-        vals[tid] = v;
-        __syncthreads();
-        if (warp == 0) {
-            const int cnt = min(1024, ns - base);
-            for (int b = 0; b < cnt; b += 32) {
-                const float mine = vals[b + lane];
-#pragma unroll
-                for (int q = 0; q < 32; ++q) k = k + __shfl_sync(0xffffffffu, mine, q);
-            }
-        }
-        __syncthreads();
-    }
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
-    if (lane == 0) part[warp] = c;
-    __syncthreads();
-    if (tid == 0) {
-        long long tot = 0;
-        for (int w = 0; w < 32; ++w) tot += part[w];
-        count[j * sys.T + t] = tot; cost[j * sys.T + t] = k;
-    }
+    totals_block(sys, blockIdx.x, 0, sys.S, TotalsPairRec{chosen_acc + j * sys.S, chosen + j * sys.S}, count + j * sys.T, cost + j * sys.T);
 }
 
 }  // namespace wva

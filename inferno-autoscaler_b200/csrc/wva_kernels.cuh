@@ -2224,28 +2224,27 @@ __global__ void k_solve_unlimited(DevSystem sys, int s0, int ns, DevAllocs pairs
     store_alloc(chosen, (size_t)s, minKey >= 0 ? load_alloc(pairs, (size_t)s * sys.A + minKey) : empty_alloc());
 }
 
-// System.AllocateByType (system.go:271-300) over servers [s0, s0+ns): one block per accelerator
-// type.  The float32 cost sum keeps a fixed order (ascending server index): the block stages 1024
+// System.AllocateByType (system.go:271-300) of type t over servers [s0, s0+ns), one block of 1024 threads.
+// The float32 cost sum keeps a fixed order (ascending server index): the block stages 1024
 // servers' contributions in shared memory in parallel, then warp 0 adds them in order (a server
 // of another type contributes +0, which leaves a float32 sum that started at +0 unchanged).
 // The int64 unit counts wrap and are associative: plain tree reduction.
-// totals = { long long count[T]; float cost[T] }.
-__global__ void __launch_bounds__(1024) k_totals(DevSystem sys, int s0, int ns, const int* __restrict__ chosen_acc, DevAllocs chosen,
-                                                 long long* __restrict__ count, float* __restrict__ cost) {
+// Rec reads server s's chosen record: chosen(s), and for a chosen server acc(s), replicas(s), cost(s).
+template <class Rec>
+__device__ __forceinline__ void totals_block(const DevSystem& sys, int t, int s0, int ns, const Rec& rec, long long* count, float* cost) {
     __shared__ float vals[1024];
     __shared__ long long part[32];
-    const int t = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     long long c = 0; float k = 0.0f;
     for (int base = 0; base < ns; base += 1024) {
         const int s = s0 + base + tid;
         float v = 0.0f;
-        if (base + tid < ns && chosen_acc[s] >= 0) {
-            const int gi = chosen.acc[s];
+        if (base + tid < ns && rec.chosen(s)) {
+            const int gi = rec.acc(s);
             const int m = sys.srv_model[s];
             if (gi >= 0 && m >= 0 && sys.acc_type[gi] == t) {
-                c += go_muli(go_muli(chosen.num_replicas[s], num_instances(sys, m, gi)), (long long)sys.acc_multiplicity[gi]);
-                v = chosen.cost[s];
+                c += go_muli(go_muli(rec.replicas(s), num_instances(sys, m, gi)), (long long)sys.acc_multiplicity[gi]);
+                v = rec.cost(s);
             }
         }
         vals[tid] = v;
@@ -2268,6 +2267,21 @@ __global__ void __launch_bounds__(1024) k_totals(DevSystem sys, int s0, int ns, 
         for (int w = 0; w < 32; ++w) tot += part[w];
         count[t] = tot; cost[t] = k;
     }
+}
+
+// the chosen records of wva_solve: chosen_acc[s] >= 0 marks a chosen server
+struct TotalsSoa {
+    const int* __restrict__ chosen_acc; DevAllocs rec;
+    __device__ bool chosen(int s) const { return chosen_acc[s] >= 0; }
+    __device__ int acc(int s) const { return rec.acc[s]; }
+    __device__ long long replicas(int s) const { return rec.num_replicas[s]; }
+    __device__ float cost(int s) const { return rec.cost[s]; }
+};
+
+// totals = { long long count[T]; float cost[T] }: one block per accelerator type
+__global__ void __launch_bounds__(1024) k_totals(DevSystem sys, int s0, int ns, const int* __restrict__ chosen_acc, DevAllocs chosen,
+                                                 long long* __restrict__ count, float* __restrict__ cost) {
+    totals_block(sys, blockIdx.x, s0, ns, TotalsSoa{chosen_acc, chosen}, count, cost);
 }
 
 // Sum the per-rank partial totals of a sharded run in rank order (deterministic, unlike a ring or

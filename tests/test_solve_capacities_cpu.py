@@ -120,41 +120,3 @@ def test_c99_declarations_link_and_reject_null(wva):
         out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0 and "solve_capacities c99: ok" in out.stdout, out.stdout + out.stderr
 
-
-def test_scan_pass_copies_differ_only_where_expected():
-    """greedy_scan_pass (k_greedy_scan_multi) is a copy of k_greedy_scan's pass: the two bodies may differ only in the
-    context setup, the capacity source, the unallocated list's owner, the group slot and the stats write"""
-    import difflib
-    src = open(os.path.join(ROOT, "inferno-autoscaler_b200", "csrc", "wva_greedy_scan.cuh")).read()
-
-    def body(start):
-        i = src.index(start)
-        return [ln.strip() for ln in src[src.index("{", i):src.index("\n}\n", i)].split("\n") if ln.strip()]
-
-    scan = body("__global__ void __launch_bounds__(32) k_greedy_scan(")
-    pas = body("__device__ __forceinline__ void greedy_scan_pass(")
-    diff = sorted(ln for ln in difflib.unified_diff(scan, pas, lineterm="", n=0)
-                  if ln[:1] in "+-" and not ln.startswith(("+++", "---")))
-    assert diff == sorted([
-        "-extern __shared__ __align__(16) unsigned char greedy_pool[];",
-        "-__shared__ long long avail[256];",
-        "-__shared__ long long usum[256];",
-        "-if (blockIdx.x != 0) return;",
-        "-const int lane = threadIdx.x;",
-        "+const int lane = c.lane;",
-        "+const DevSystem& sys = c.sys;",
-        "-GreedyCtx c; c.sys = sys; c.pairs = pairs; c.g = g; c.chosen = chosen; c.avail = avail; c.usum = usum; c.lane = lane;",
-        "-c.g.smemBytes = g.smemBytes - (int)doneBytes;",
-        "-for (int t = lane; t < sys.T; t += 32) avail[t] = sys.type_capacity[t];",
-        "+c.g.smemBytes = c.g.smemBytes - (int)doneBytes;",
-        "+for (int t = lane; t < sys.T; t += 32) c.avail[t] = capacity[t];",
-        "-greedy_best_effort(c, g.unalloc, nUn, policy);",
-        "+greedy_best_effort(c, c.g.unalloc, nUn, policy);",
-        "-const int g0 = base + lo;",
-        "+const int g0 = groupSlot(base + lo);",
-        "-greedy_best_effort(c, g.unalloc, nUn, policy);",
-        "+greedy_best_effort(c, c.g.unalloc, nUn, policy);",
-        "-if (lane == 0) { g.stats[0] = (unsigned long long)nEv + (nGroups << 32); g.stats[1] = nBatches + (nPopped << 32); "
-        "g.stats[2] = cycScan; g.stats[3] = cycBest; }",
-        "+st[0] = (unsigned long long)nEv + (nGroups << 32); st[1] = nBatches + (nPopped << 32); st[2] = cycScan; st[3] = cycBest;",
-    ]), diff
