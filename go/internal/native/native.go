@@ -348,8 +348,9 @@ func (c *Context) PairsAtArrivalRates(rpm []float32, nLoads int, wantPlane bool)
 		"wva_analyze_pairs_loads")
 }
 
-// CapacityScenarios is what SolveAtCapacities returns for nVec capacity vectors: Acc[j*S+s] and Chosen[j*S+s] are the
-// limited solve's decision and chosen record (after best-effort scaling, Feasible = 1 where Acc >= 0) under vector j,
+// CapacityScenarios is what SolveAtCapacities returns for nVec capacity vectors (and SolveAtArrivalRates for nLoads
+// arrival-rate scenarios): Acc[j*S+s] and Chosen[j*S+s] are the limited solve's decision and chosen record (after
+// best-effort scaling, Feasible = 1 where Acc >= 0) under vector (scenario) j,
 // Count[j*T+t] and Cost[j*T+t] its AllocateByType totals over every server.
 type CapacityScenarios struct {
 	Acc    []int32
@@ -387,6 +388,32 @@ func (c *Context) SolveAtCapacities(capacity []int64, nVec int, delayedBestEffor
 	}
 	return out, c.err(C.wva_solve_capacities(c.ctx, &spec, C.int32_t(nVec), i64p(capacity), i32p(out.Acc), pairRecs(out.Chosen),
 		i64p(out.Count), f32p(out.Cost)), "wva_solve_capacities")
+}
+
+// SolveAtArrivalRates runs the limited solve once per arrival-rate scenario -- rpm[srv*nLoads+j] is server srv's
+// ServerLoadSpec.ArrivalRate (req/min) in scenario j, 1 <= nLoads <= 8192, the layout of PairsAtArrivalRates -- under the
+// image's capacities in one call: scenario j gives what UpdateServers with those rates, AnalyzePairs, a limited Solve and
+// AllocateByType would, in CapacityScenarios' layout with j indexing scenarios.  QueueAnalyzer.Size runs once per pair
+// and chunk.  The image, pair records and last Solve's decisions are left as they were; no AnalyzePairs is needed before
+// it.  The context must hold every server (no shard).
+func (c *Context) SolveAtArrivalRates(rpm []float32, nLoads int, delayedBestEffort bool, policy int) (*CapacityScenarios, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var S, A, M, T C.int32_t
+	if err := c.err(C.wva_system_dims(c.ctx, &S, &A, &M, &T), "wva_system_dims"); err != nil {
+		return nil, err
+	}
+	if nLoads < 1 || len(rpm) != int(S)*nLoads {
+		return nil, fmt.Errorf("SolveAtArrivalRates: rpm needs S*nLoads = %d*%d rates, got %d", int(S), nLoads, len(rpm))
+	}
+	out := &CapacityScenarios{Acc: make([]int32, nLoads*int(S)), Chosen: make([]PairRec, nLoads*int(S)),
+		Count: make([]int64, nLoads*int(T)), Cost: make([]float32, nLoads*int(T))}
+	spec := C.wva_optimizer_spec{unlimited: 0, delayed_best_effort: 0, saturation_policy: C.int32_t(policy)}
+	if delayedBestEffort {
+		spec.delayed_best_effort = 1
+	}
+	return out, c.err(C.wva_solve_loads(c.ctx, &spec, C.int32_t(nLoads), f32p(rpm), i32p(out.Acc), pairRecs(out.Chosen),
+		i64p(out.Count), f32p(out.Cost)), "wva_solve_loads")
 }
 
 // QueueConfig is wva_queue_config; Metrics is wva_metrics (analyzer.AnalysisMetrics).

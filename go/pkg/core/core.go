@@ -553,6 +553,16 @@ func (s *System) SolveAtCapacities(spec *config.OptimizerSpec, capacity []int64,
 	return s.ctx.SolveAtCapacities(capacity, nVec, spec.DelayedBestEffort, int(config.SaturatedAllocationPolicyEnum(spec.SaturationPolicy)))
 }
 
+// SolveAtArrivalRates runs the limited solve of spec under each of nLoads arrival-rate scenarios (rpm[srv*nLoads+j]:
+// server srv's ArrivalRate in req/min in scenario j, servers in the uploaded image's order) on the system's capacities in
+// one native call.  Server allocations, loads, candidates and capacities are left as they were.
+func (s *System) SolveAtArrivalRates(spec *config.OptimizerSpec, rpm []float32, nLoads int) (*native.CapacityScenarios, error) {
+	if err := s.upload(); err != nil {
+		return nil, err
+	}
+	return s.ctx.SolveAtArrivalRates(rpm, nLoads, spec.DelayedBestEffort, int(config.SaturatedAllocationPolicyEnum(spec.SaturationPolicy)))
+}
+
 // AllocateByType (system.go:271-300)
 func (s *System) AllocateByType() {
 	s.allocationByType = map[string]*AllocationByType{}

@@ -59,6 +59,15 @@ func (s *Solver) SolveAtCapacities(capacity []int64, nVec int) (*native.Capacity
 	return core.TheSystem.SolveAtCapacities(&spec, capacity, nVec)
 }
 
+// SolveAtArrivalRates answers "what would SolveGreedy decide at these loads?" for nLoads arrival-rate scenarios at once
+// (rpm[srv*nLoads+j]: server srv's ArrivalRate in req/min in scenario j) on the system's capacities, without changing
+// the system's allocations, loads or capacities.
+func (s *Solver) SolveAtArrivalRates(rpm []float32, nLoads int) (*native.CapacityScenarios, error) {
+	spec := *s.optimizerSpec
+	spec.Unlimited = false
+	return core.TheSystem.SolveAtArrivalRates(&spec, rpm, nLoads)
+}
+
 type Optimizer struct {
 	spec             *config.OptimizerSpec
 	solver           *Solver

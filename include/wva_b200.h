@@ -475,6 +475,46 @@ int wva_solve_capacities_counters(const wva_ctx* ctx, uint64_t out[4]);
  * span several chunks.  Results do not depend on it. */
 int wva_solve_capacities_set_budget(wva_ctx* ctx, int64_t bytes);
 
+/* Limited-capacity solve over a matrix of arrival-rate scenarios: arrival_rpm[s * n_l + j] is server s's
+ * ServerLoadSpec.ArrivalRate (requests per minute) in scenario j, 1 <= n_l <= 8192 -- the layout of
+ * wva_analyze_pairs_loads, so one matrix serves both calls.  Scenario j's outputs are what this library returns after
+ * wva_system_update_servers(0, S, rows) with the uploaded rows and srv_arrival_rpm[s] = arrival_rpm[s * n_l + j], then
+ * wva_analyze_pairs, a limited wva_solve(spec), wva_solution_fetch and wva_allocate_by_type, under the image's own
+ * type_capacity:
+ *   chosen_acc [n_l * S], index j * S + s, or NULL: the solve's chosen_acc;
+ *   chosen     [n_l * S], or NULL: the solve's chosen record after best-effort scaling (greedy.go:208-212, :302-311) with
+ *              feasible = 1 where chosen_acc >= 0; elsewhere the empty record wva_solution_fetch gives (acc = -1,
+ *              feasible = 0, pad = 0);
+ *   type_count / type_cost [n_l * T], index j * T + t, or NULL: AllocateByType over all S servers, the float32 cost summed
+ *              in ascending server index from +0 (wva_solve_capacities's totals).
+ * The rates mean what they mean to wva_analyze_pairs_loads: +0 and -0 give the zero-load records, a negative rate gives
+ * nil records, a positive rate whose totalRate is 0 on a server with MinNumReplicas <= 0 gives the empty record.  The
+ * solve means what limited wva_solve means: every saturation policy, both best-effort schedules, negative capacities,
+ * wrapped int64 counts, NaN / +-Inf values, T <= 256, every solver path (wva_solve_set_ranked).  QueueAnalyzer.Size runs
+ * once per pair and chunk whatever the chunk's scenario count is.  The candidate values depend on the load, so each
+ * scenario gets its own candidate order and sorted static order; the scan pass then runs once per scenario, one warp
+ * each, side by side.  Shapes the scan path does not take, and wva_solve_set_ranked < 2, run the ranked-queue or heap
+ * kernel once per scenario instead (slower, same results).  Scenarios are staged in chunks whose pair records, greedy
+ * buffers and outputs fit 2^28 bytes (one scenario at least); each chunk is copied out before the next starts.
+ * The call sizes its own records from the image: it needs no wva_analyze_pairs before it, and works after a limited
+ * wva_solve has scaled the resident records.  Nothing that other calls read changes: the resident image
+ * (srv_arrival_rpm and type_capacity included), the pair records and feasible flags and whether they are valid, the last
+ * wva_solve's decisions and whether it ran, wva_solve_greedy_path and wva_solve_stats, the totals buffer, sweep results,
+ * and the counters of wva_analyze_pairs_loads and wva_solve_capacities.
+ * Errors, which change nothing: WVA_EINVAL for spec == NULL, spec->unlimited != 0 (the unlimited choice is
+ * wva_analyze_pairs_loads's best record), n_l out of range, arrival_rpm == NULL while S > 0, a NaN rate, T > 256 or
+ * S * A >= 2^31; WVA_ESTATE before any upload, or when the context's shard is not every server. */
+#define WVA_SOLVE_MAX_LOADS 8192
+int wva_solve_loads(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n_l, const float* arrival_rpm, int32_t* chosen_acc,
+                    wva_pair_rec* chosen, int64_t* type_count, float* type_cost);
+/* Counters of the last wva_solve_loads: {scenario chunks, solver path run (3 scan, 2 ranked queue, 1 heap, 0 when S = 0),
+ * pairs that reached QueueAnalyzer.Size (summed over chunks), (pair, scenario) items that reached the final Analyze,
+ * items sent to the materialised-p[] path, SM cycles of the slowest scenario's scan pass (scan path, else 0)}. */
+int wva_solve_loads_counters(const wva_ctx* ctx, uint64_t out[6]);
+/* Test hook: staging budget of wva_solve_loads in bytes (0 restores the default 2^28), so that small images can span
+ * several chunks.  Results do not depend on it. */
+int wva_solve_loads_set_budget(wva_ctx* ctx, int64_t bytes);
+
 /* Replaces System.AllocateByType (pkg/core/system.go:271-300): per accelerator type
  * count += replicas*numInstances*multiplicity, cost += alloc.cost over this rank's shard.
  * The sums are left in a device buffer (wva_type_totals_device) so the host can run the

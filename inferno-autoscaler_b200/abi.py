@@ -126,6 +126,7 @@ PAIR_REC_DTYPE = np.dtype(dict(
 PAIRS_MAX_BATCH = PAIRS_MAX_BATCHES = 8192
 PAIRS_MAX_LOADS = 8192          # scenarios of one wva_analyze_pairs_loads call
 SOLVE_MAX_CAPACITIES = 8192     # capacity vectors of one wva_solve_capacities call
+SOLVE_MAX_LOADS = 8192          # arrival-rate scenarios of one wva_solve_loads call
 
 assert C.sizeof(PairRec) == PAIR_REC_DTYPE.itemsize == 48
 assert C.sizeof(Metrics) == METRICS_DTYPE.itemsize == 32

@@ -34,6 +34,7 @@ EXPORTS = [
     "wva_analyze_pairs_batches", "wva_pairs_batches_counters", "wva_group_analyze_pairs_batches", "wva_shard_info",
     "wva_analyze_pairs_loads", "wva_pairs_loads_counters", "wva_group_analyze_pairs_loads",
     "wva_solve_capacities", "wva_solve_capacities_counters", "wva_solve_capacities_set_budget", "wva_group_solve_capacities",
+    "wva_solve_loads", "wva_solve_loads_counters", "wva_solve_loads_set_budget",
 ]
 
 
@@ -145,6 +146,9 @@ def lib():
         L.wva_solve_capacities_counters.argtypes = [vp, C.POINTER(u64)]
         L.wva_solve_capacities_set_budget.argtypes = [vp, i64]
         L.wva_group_solve_capacities.argtypes = [vp, C.POINTER(abi.OptimizerSpec), i32, abi.i64p, abi.i32p, vp, abi.i64p, abi.f32p]
+        L.wva_solve_loads.argtypes = [vp, C.POINTER(abi.OptimizerSpec), i32, abi.f32p, abi.i32p, vp, abi.i64p, abi.f32p]
+        L.wva_solve_loads_counters.argtypes = [vp, C.POINTER(u64)]
+        L.wva_solve_loads_set_budget.argtypes = [vp, i64]
         if L.wva_abi_version() != abi.ABI_VERSION:
             raise ImportError("libwva_b200.so ABI version mismatch")
         _lib = L
@@ -542,6 +546,39 @@ class Context:
     def solve_capacities_set_budget(self, nbytes):
         """staging budget of solve_capacities in bytes (0: the default 2^28)"""
         self._ck(lib().wva_solve_capacities_set_budget(self._h, int(nbytes)))
+
+    def solve_loads(self, rpm, delayed_best_effort=False, policy=abi.POLICY_NONE, download=True):
+        """Limited solve under each arrival-rate scenario of rpm [S, n_l] (req/min, the layout of analyze_pairs_loads) in
+        one call, under the image's capacities; the resident image and results stay as they are.  Returns (chosen_acc
+        [n_l, S], recs [n_l, S] of abi.PAIR_REC_DTYPE, count [n_l, T], cost [n_l, T]): row j is what update_servers with
+        rates rpm[:, j], analyze_pairs, a limited solve, solution_fetch and allocate_by_type give.  None when download is
+        False."""
+        img = self.image
+        r = np.ascontiguousarray(rpm, dtype=np.float32)
+        if r.ndim != 2 or r.shape[0] != img.S:
+            raise ValueError("rpm must be shaped [S, n_l]")
+        n_l = r.shape[1]
+        spec = abi.OptimizerSpec(0, 1 if delayed_best_effort else 0, int(policy))
+        if not download:
+            self._ck(lib().wva_solve_loads(self._h, C.byref(spec), n_l, abi.ptr(r, C.c_float), None, None, None, None))
+            return None
+        acc = np.full((n_l, img.S), -1, dtype=np.int32)
+        recs = np.zeros((n_l, img.S), dtype=abi.PAIR_REC_DTYPE)
+        count = np.zeros((n_l, img.T), dtype=np.int64)
+        cost = np.zeros((n_l, img.T), dtype=np.float32)
+        self._ck(lib().wva_solve_loads(self._h, C.byref(spec), n_l, abi.ptr(r, C.c_float), abi.ptr(acc, C.c_int32), recs.ctypes.data,
+                                       abi.ptr(count, C.c_int64), abi.ptr(cost, C.c_float)))
+        return acc, recs, count, cost
+
+    def solve_loads_counters(self):
+        """counters of the last solve_loads"""
+        v = (C.c_uint64 * 6)()
+        self._ck(lib().wva_solve_loads_counters(self._h, v))
+        return dict(chunks=v[0], path=v[1], sized_pairs=v[2], analyzed=v[3], materialised=v[4], max_cycles=v[5])
+
+    def solve_loads_set_budget(self, nbytes):
+        """staging budget of solve_loads in bytes (0: the default 2^28)"""
+        self._ck(lib().wva_solve_loads_set_budget(self._h, int(nbytes)))
 
     def solution_fetch(self):
         """The decisions of the last solve (also one made with download=False): (chosen_acc[S], AllocArrays[S])."""

@@ -211,6 +211,10 @@ struct wva_ctx {
     DevBuf capShared, capSlots, capChunk, capPairs;
     size_t cap_budget = (size_t)1 << 28;
     uint64_t cap_counters[4] = {0, 0, 0, 0};
+    // wva_solve_loads: chunk buffer of its own (pair sizing runs in wva_analyze_pairs_loads's scratch), budget, counters
+    DevBuf slChunk;
+    size_t sl_budget = (size_t)1 << 28;
+    uint64_t sl_counters[6] = {0, 0, 0, 0, 0, 0};
 
     // grid
     DevBuf keys, bestDev, cube, status, counters, gridSlow, gridSlowCount, faultList, faultCount;
@@ -442,7 +446,7 @@ void wva_ctx_destroy(wva_ctx* ctx) {
                       &ctx->pbBatch, &ctx->pbSlow, &ctx->pbScratch, &ctx->pbScratchOff,
                       &ctx->pbPlane, &ctx->pbBest, &ctx->pbCount,
                       &ctx->plRpm, &ctx->plSlow, &ctx->plScratch, &ctx->plScratchOff, &ctx->plPlane, &ctx->plBest,
-                      &ctx->plCount, &ctx->plTabOff, &ctx->plTabs};
+                      &ctx->plCount, &ctx->plTabOff, &ctx->plTabs, &ctx->slChunk};
     for (DevBuf* b : bufs) b->release();
     ctx->staging.release();
     cudaEventDestroy(ctx->ev0);
@@ -890,6 +894,92 @@ int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]) {
     return WVA_OK;
 }
 
+// Pair sizing of servers [f, f + nss) under nL scenarios: the rates are on the device already, rpm[(s - f) * nL + j], and
+// record (s, j, a) lands at plane[((s - f) * nL + j) * A + a].  The rate tables are planned here from N under a positive
+// load (the plan of wva_analyze_pairs follows the uploaded rates and gives a zero-load server no table); k_pairs_loads
+// sizes each pair once and k_pairs_loads_literal re-runs the items it sent to the materialised path.  Scratch and
+// counters are wva_analyze_pairs_loads's (ctx->plCount: [0, 4) slow-list length, [8, 56) k_pairs_loads's counters,
+// zeroed by the caller); nSlow grows by the items of the materialised path.  Returns with the stream drained.
+static int pairs_loads_run(wva_ctx* ctx, int f, int nss, int n_l, const float* dRpm, wva_pair_rec* dPlane, uint64_t& nSlow) {
+    const int A = ctx->A;
+    CK(ctx->plSlow.ensure((size_t)nss * A * n_l * 8));
+    CK(ctx->plTabOff.ensure((size_t)nss * A * 8));
+    char* cnt = ctx->plCount.as<char>();
+    int* slowCount = reinterpret_cast<int*>(cnt);
+    unsigned long long* counters = reinterpret_cast<unsigned long long*>(cnt + 8);
+    unsigned long long* dSlow = ctx->plSlow.as<unsigned long long>();
+    const int warpsPerBlock = WVA_PAIRS_WARP_THREADS / 32;
+    const long long budget = (2LL << 30) / 16;           // at most 2 GB of tables, as wva_analyze_pairs
+    std::vector<long long> nPair, offs;
+    std::vector<unsigned long long> items;
+    std::vector<long long> soffs;
+    const int nPairs = nss * A;
+    // table plan: the warp's shared-memory slice up to 3072 entries, HBM above that under the budget, the
+    // materialised path beyond it or above 2^26 entries
+    nPair.resize((size_t)nPairs);
+    offs.resize((size_t)nPairs);
+    long long maxN = 0, total = 0;
+    for (int i = 0; i < nPairs; ++i) {
+        const long long N = host_pair_n(ctx, f + i / A, i % A);
+        nPair[(size_t)i] = N;
+        if (N > maxN && N <= (1LL << 26)) maxN = N;
+    }
+    const long long inSmem = ctx->pairs_smem ? (maxN < 3072 ? maxN : 3072) : 0;
+    for (int i = 0; i < nPairs; ++i) {
+        const long long N = nPair[(size_t)i];
+        if (N <= 0 || N <= inSmem) { offs[(size_t)i] = 0; continue; }
+        if (N > (1LL << 26) || total + N > budget) { offs[(size_t)i] = -1; continue; }
+        offs[(size_t)i] = total; total += N;
+    }
+    CK(ctx->plTabs.ensure((size_t)(total ? total : 1) * 16));
+    CK(cudaMemcpyAsync(ctx->plTabOff.p, offs.data(), (size_t)nPairs * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(slowCount, 0, 4, ctx->stream));
+    const int smemEntries = (int)inSmem;
+    const size_t smemBytes = (size_t)smemEntries * 16 * warpsPerBlock;
+    if (smemBytes > 48 * 1024) CK(cudaFuncSetAttribute(k_pairs_loads, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+    k_pairs_loads<<<(nPairs + warpsPerBlock - 1) / warpsPerBlock, WVA_PAIRS_WARP_THREADS, smemBytes, ctx->stream>>>(
+        ctx->dsys, f, nPairs, n_l, dRpm, ctx->plTabOff.as<long long>(), ctx->plTabs.as<double2>(), smemEntries, dPlane, dSlow,
+        slowCount, counters);
+    LAUNCH_CHECK();
+    int slow = 0;
+    CK(cudaMemcpyAsync(&slow, slowCount, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (slow > 0) {
+        // items whose chain hit an overflow-rescale branch, or whose pair has no usable table: p[] in HBM.  A pair
+        // can send all n_l of its items here, so they run in chunks whose scratch fits half the free memory: the call
+        // fails only when a single item does not fit, where wva_analyze_pairs fails too.
+        items.resize((size_t)slow);
+        soffs.resize((size_t)slow);
+        CK(cudaMemcpy(items.data(), dSlow, (size_t)slow * 8, cudaMemcpyDeviceToHost));
+        size_t freeB = 0, totB = 0;
+        CK(cudaMemGetInfo(&freeB, &totB));
+        const size_t capB = std::max(freeB / 2, ctx->plScratch.cap);
+        for (int i0 = 0; i0 < slow;) {
+            long long stotal = 0;
+            int i1 = i0;
+            for (; i1 < slow; ++i1) {
+                const unsigned long long it = items[(size_t)i1];
+                const long long N = nPair[(size_t)((it / (unsigned long long)A) / (unsigned long long)n_l * A + it % (unsigned long long)A)];
+                if (N > (1LL << 32)) return fail(ctx, WVA_EINVAL, "pair needs the materialised path with an unreasonably large batch size");
+                if (i1 > i0 && (size_t)(stotal + 11 * N + 1) * 8 > capB) break;
+                soffs[(size_t)(i1 - i0)] = stotal; stotal += 11 * N + 1;
+            }
+            if ((size_t)stotal * 8 > capB) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
+            const int n = i1 - i0;
+            CK(ctx->plScratch.ensure((size_t)stotal * 8));
+            CK(ctx->plScratchOff.ensure((size_t)n * 8));
+            CK(cudaMemcpyAsync(ctx->plScratchOff.p, soffs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+            k_pairs_loads_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, n_l, dRpm, dSlow + i0, n, ctx->plScratch.as<double>(),
+                                                                        ctx->plScratchOff.as<long long>(), dPlane, counters);
+            LAUNCH_CHECK();
+            CK(cudaStreamSynchronize(ctx->stream));      // the next chunk reuses the scratch and its offsets
+            i0 = i1;
+        }
+        nSlow += (uint64_t)slow;
+    }
+    return WVA_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Pair sizing over a matrix of arrival-rate scenarios.  Per slice of servers: the slice's rows of rates go to the
 // device, k_pairs_loads sizes each pair once and writes its record under every scenario, k_pairs_loads_literal re-runs
@@ -913,101 +1003,28 @@ int wva_analyze_pairs_loads(wva_ctx* ctx, int32_t n_l, const float* arrival_rpm,
     if (ns == 0) return WVA_OK;
     const size_t recBytes = perServer * sizeof(wva_pair_rec);
     const int slice = (int)std::max<size_t>(1, std::min<size_t>((size_t)ns, ((size_t)1 << 28) / recBytes));
-    const size_t maxItems = (size_t)slice * perServer;
     CK(ctx->plRpm.ensure((size_t)slice * n_l * 4));
-    CK(ctx->plSlow.ensure(maxItems * 8));
     CK(ctx->plPlane.ensure((size_t)slice * recBytes));
     CK(ctx->plBest.ensure((size_t)slice * n_l * sizeof(wva_pair_rec)));
-    CK(ctx->plTabOff.ensure((size_t)slice * A * 8));
     CK(ctx->plCount.ensure(64));
-    // [0, 4) slow-list length, [8, 56) k_pairs_loads's counters
-    char* cnt = ctx->plCount.as<char>();
-    int* slowCount = reinterpret_cast<int*>(cnt);
-    unsigned long long* counters = reinterpret_cast<unsigned long long*>(cnt + 8);
-    CK(cudaMemsetAsync(cnt, 0, 64, ctx->stream));
+    CK(cudaMemsetAsync(ctx->plCount.p, 0, 64, ctx->stream));
+    const unsigned long long* counters = reinterpret_cast<const unsigned long long*>(ctx->plCount.as<char>() + 8);
     float* dRpm = ctx->plRpm.as<float>();
     wva_pair_rec* dPlane = ctx->plPlane.as<wva_pair_rec>();
     wva_pair_rec* dBest = ctx->plBest.as<wva_pair_rec>();
-    unsigned long long* dSlow = ctx->plSlow.as<unsigned long long>();
-    const int warpsPerBlock = WVA_PAIRS_WARP_THREADS / 32;
-    const long long budget = (2LL << 30) / 16;           // at most 2 GB of tables, as wva_analyze_pairs
-    std::vector<long long> nPair, offs;
-    std::vector<unsigned long long> items;
-    std::vector<long long> soffs;
     uint64_t nSlices = 0, nSlow = 0;
+    int rc = WVA_OK;
     for (int f = ctx->s0; f < ctx->s0 + ns; f += slice) {
         const int nss = std::min(slice, ctx->s0 + ns - f);
-        const int nPairs = nss * A;
         const size_t hs = (size_t)(f - ctx->s0);
-        // table plan: the warp's shared-memory slice up to 3072 entries, HBM above that under the budget, the
-        // materialised path beyond it or above 2^26 entries
-        nPair.resize((size_t)nPairs);
-        offs.resize((size_t)nPairs);
-        long long maxN = 0, total = 0;
-        for (int i = 0; i < nPairs; ++i) {
-            const long long N = host_pair_n(ctx, f + i / A, i % A);
-            nPair[(size_t)i] = N;
-            if (N > maxN && N <= (1LL << 26)) maxN = N;
-        }
-        const long long inSmem = ctx->pairs_smem ? (maxN < 3072 ? maxN : 3072) : 0;
-        for (int i = 0; i < nPairs; ++i) {
-            const long long N = nPair[(size_t)i];
-            if (N <= 0 || N <= inSmem) { offs[(size_t)i] = 0; continue; }
-            if (N > (1LL << 26) || total + N > budget) { offs[(size_t)i] = -1; continue; }
-            offs[(size_t)i] = total; total += N;
-        }
-        CK(ctx->plTabs.ensure((size_t)(total ? total : 1) * 16));
-        CK(cudaMemcpyAsync(ctx->plTabOff.p, offs.data(), (size_t)nPairs * 8, cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(dRpm, arrival_rpm + hs * n_l, (size_t)nss * n_l * 4, cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaMemsetAsync(slowCount, 0, 4, ctx->stream));
-        const int smemEntries = (int)inSmem;
-        const size_t smemBytes = (size_t)smemEntries * 16 * warpsPerBlock;
-        if (smemBytes > 48 * 1024) CK(cudaFuncSetAttribute(k_pairs_loads, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
-        k_pairs_loads<<<(nPairs + warpsPerBlock - 1) / warpsPerBlock, WVA_PAIRS_WARP_THREADS, smemBytes, ctx->stream>>>(
-            ctx->dsys, f, nPairs, n_l, dRpm, ctx->plTabOff.as<long long>(), ctx->plTabs.as<double2>(), smemEntries, dPlane, dSlow,
-            slowCount, counters);
-        LAUNCH_CHECK();
-        int slow = 0;
-        CK(cudaMemcpyAsync(&slow, slowCount, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        if (slow > 0) {
-            // items whose chain hit an overflow-rescale branch, or whose pair has no usable table: p[] in HBM.  A pair
-            // can send all n_l of its items here, so they run in chunks whose scratch fits half the free memory: the call
-            // fails only when a single item does not fit, where wva_analyze_pairs fails too.
-            items.resize((size_t)slow);
-            soffs.resize((size_t)slow);
-            CK(cudaMemcpy(items.data(), dSlow, (size_t)slow * 8, cudaMemcpyDeviceToHost));
-            size_t freeB = 0, totB = 0;
-            CK(cudaMemGetInfo(&freeB, &totB));
-            const size_t capB = std::max(freeB / 2, ctx->plScratch.cap);
-            for (int i0 = 0; i0 < slow;) {
-                long long stotal = 0;
-                int i1 = i0;
-                for (; i1 < slow; ++i1) {
-                    const unsigned long long it = items[(size_t)i1];
-                    const long long N = nPair[(size_t)((it / (unsigned long long)A) / (unsigned long long)n_l * A + it % (unsigned long long)A)];
-                    if (N > (1LL << 32)) return fail(ctx, WVA_EINVAL, "pair needs the materialised path with an unreasonably large batch size");
-                    if (i1 > i0 && (size_t)(stotal + 11 * N + 1) * 8 > capB) break;
-                    soffs[(size_t)(i1 - i0)] = stotal; stotal += 11 * N + 1;
-                }
-                if ((size_t)stotal * 8 > capB) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-                const int n = i1 - i0;
-                CK(ctx->plScratch.ensure((size_t)stotal * 8));
-                CK(ctx->plScratchOff.ensure((size_t)n * 8));
-                CK(cudaMemcpyAsync(ctx->plScratchOff.p, soffs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-                k_pairs_loads_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, n_l, dRpm, dSlow + i0, n, ctx->plScratch.as<double>(),
-                                                                            ctx->plScratchOff.as<long long>(), dPlane, counters);
-                LAUNCH_CHECK();
-                CK(cudaStreamSynchronize(ctx->stream));      // the next chunk reuses the scratch and its offsets
-                i0 = i1;
-            }
-            nSlow += (uint64_t)slow;
-        }
+        rc = pairs_loads_run(ctx, f, nss, n_l, dRpm, dPlane, nSlow);
+        if (rc != WVA_OK) return rc;
         k_pairs_plane_best<<<(nss * n_l + 3) / 4, 128, 0, ctx->stream>>>(dPlane, nss * n_l, A, dBest);
         LAUNCH_CHECK();
         if (plane) CK(cudaMemcpyAsync(plane + hs * perServer, dPlane, (size_t)nss * recBytes, cudaMemcpyDeviceToHost, ctx->stream));
         if (best) CK(cudaMemcpyAsync(best + hs * n_l, dBest, (size_t)nss * n_l * sizeof(wva_pair_rec), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));       // also releases offs, soffs and the slice's buffers for the next slice
+        CK(cudaStreamSynchronize(ctx->stream));       // the next slice reuses the slice's buffers
         ++nSlices;
     }
     unsigned long long dev[6];
@@ -1694,7 +1711,9 @@ struct GreedyPlan {
     size_t nS, nSA, n2, doneBytes;
     int path;
 };
-static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
+// greedy_carve lays the buffers out from b (b == nullptr: only the bytes they take are returned); greedy_order fills them
+// from the candidate records `pairs` / `feasible` (wva_solve_loads hands it each scenario's records).
+static size_t greedy_carve(const wva_ctx* ctx, char* b, GreedyPlan& p) {
     const int S = ctx->S, A = ctx->A;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
@@ -1717,8 +1736,9 @@ static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
         o_ka = take(n2 * 8); o_kb = take(n2 * 4); o_ks = take(n2 * 4); o_pos = take(nSA * 4); o_sn = take(nSA * 4);
         o_rec = take(n2 * 16); o_np = take(n2 * 8); o_ge = take(n2 * 4); o_gb = take(n2 * 4); o_top = take((n2 + 1) * 4); o_succ = take(nS * 4);
     }
-    CK(buf.ensure(off));
-    char* b = buf.as<char>();
+    p.nS = nS; p.nSA = nSA; p.n2 = n2; p.doneBytes = doneBytes;
+    p.path = scannable ? 3 : rankable ? 2 : 1;
+    if (!b) return off;
     GreedyBufs& g = p.g;
     g.order = (int*)(b + o_order); g.cand = (GreedyCand*)(b + o_cand); g.upr = (long long*)(b + o_upr); g.rep = (long long*)(b + o_rep);
     g.ctype = (int*)(b + o_ct); g.nCand = (int*)(b + o_n); g.groupStart = (int*)(b + o_gs); g.groupItems = (int*)(b + o_gi);
@@ -1739,20 +1759,26 @@ static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
         gsc.ev = gr.rec; gsc.push = gr.nextPos; gsc.gbeg = gr.gbeg; gsc.stackTop = gr.top; gsc.stackBuf = gr.gend;
         gsc.nEv = g.nanFlag; gsc.n2 = (unsigned)n2;
     }
+    p.chosenKey = (int*)(b + o_key);
+    return off;
+}
+static int greedy_order(wva_ctx* ctx, const GreedyPlan& p, const DevAllocs& pairs, const unsigned char* feasible) {
+    const int S = ctx->S;
+    const GreedyBufs& g = p.g; const GreedyRank& gr = p.gr; const GreedyScan& gsc = p.gsc;
+    const size_t nS = p.nS, n2 = p.n2;
+    const bool scannable = p.path == 3, rankable = p.path == 2;
     if (!ctx->greedy_attr) {
         CK(cudaFuncSetAttribute(k_greedy_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
         CK(cudaFuncSetAttribute(k_greedy_solve_ranked, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
         CK(cudaFuncSetAttribute(k_greedy_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kGreedySmem));
         ctx->greedy_attr = true;
     }
-    int* chosenKey = (int*)(b + o_key);
-    p.chosenKey = chosenKey;
     CK(cudaMemsetAsync(g.groupStart, 0, 104 * 4, ctx->stream));
     CK(cudaMemsetAsync(g.nanFlag, 0, 8, ctx->stream));
     CK(cudaMemsetAsync(g.stats, 0, 32, ctx->stream));
-    CK(cudaMemsetAsync(chosenKey, 0xff, nS * 4, ctx->stream));
+    CK(cudaMemsetAsync(p.chosenKey, 0xff, nS * 4, ctx->stream));
     if (S > 0) {
-        k_greedy_prepare<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, ctx->pairs, ctx->feasible, g);
+        k_greedy_prepare<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, pairs, feasible, g);
         LAUNCH_CHECK();
         k_greedy_bucket_count<<<(S + 255) / 256, 256, 0, ctx->stream>>>(ctx->dsys, g);
         LAUNCH_CHECK();
@@ -1791,9 +1817,12 @@ static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
             }
         }
     }
-    p.nS = nS; p.nSA = nSA; p.n2 = n2; p.doneBytes = doneBytes;
-    p.path = scannable ? 3 : rankable ? 2 : 1;
     return WVA_OK;
+}
+static int greedy_setup(wva_ctx* ctx, DevBuf& buf, GreedyPlan& p) {
+    CK(buf.ensure(greedy_carve(ctx, nullptr, p)));
+    greedy_carve(ctx, buf.as<char>(), p);
+    return greedy_order(ctx, p, ctx->pairs, ctx->feasible);
 }
 
 // the ticket pool of the round-robin policies: a GreedyTicket and an index per server (none for the other policies)
@@ -2106,6 +2135,156 @@ int wva_solve_capacities_counters(const wva_ctx* ctx, uint64_t out[4]) {
 int wva_solve_capacities_set_budget(wva_ctx* ctx, int64_t bytes) {
     if (!ctx || bytes < 0) return WVA_EINVAL;
     ctx->cap_budget = bytes == 0 ? (size_t)1 << 28 : (size_t)bytes;
+    return WVA_OK;
+}
+
+}  // extern "C"
+
+// scenario j's records of a chunk: the fields at offset j * S * A
+static DevAllocs allocs_at(const DevAllocs& a, size_t off) {
+    DevAllocs o = a;
+    o.acc += off; o.num_replicas += off; o.batch_size += off; o.cost += off; o.value += off; o.itl += off; o.ttft += off; o.rho += off;
+    o.max_arrv += off;
+    return o;
+}
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------------------
+// Limited solve over a matrix of arrival-rate scenarios.  Per chunk of scenarios that fits the staging budget: the
+// chunk's columns of rates go to the device, pairs_loads_run sizes every pair for them (QueueAnalyzer.Size once per
+// pair), k_loads_records lays each scenario's records out as the resident ones are, and greedy_order builds each
+// scenario's candidate and static order in buffers of its own.  Then k_greedy_scan_loads runs the pass for every
+// scenario side by side (the ranked-queue or heap kernel once per scenario on the other paths), k_greedy_collect_multi
+// builds each scenario's chosen records, k_totals_multi sums the types, and the chunk is copied out.
+int wva_solve_loads(wva_ctx* ctx, const wva_optimizer_spec* spec, int32_t n_l, const float* arrival_rpm, int32_t* chosen_acc,
+                    wva_pair_rec* chosen, int64_t* type_count, float* type_cost) {
+    if (!ctx) return WVA_EINVAL;
+    if (!spec) return fail(ctx, WVA_EINVAL, "null argument");
+    if (spec->unlimited) return fail(ctx, WVA_EINVAL, "unlimited decisions are wva_analyze_pairs_loads's best records");
+    if (n_l < 1 || n_l > WVA_SOLVE_MAX_LOADS) return fail(ctx, WVA_EINVAL, "scenario count: 1 <= n_l <= 8192 required");
+    if (!ctx->have_system) return fail(ctx, WVA_ESTATE, "no system uploaded");
+    const int S = ctx->S, A = ctx->A, T = ctx->T;
+    if (S > 0 && !arrival_rpm) return fail(ctx, WVA_EINVAL, "arrival_rpm is NULL");
+    const size_t nRates = (size_t)S * (size_t)n_l;
+    for (size_t i = 0; i < nRates; ++i)
+        if (arrival_rpm[i] != arrival_rpm[i]) return fail(ctx, WVA_EINVAL, "NaN arrival rate (the reference's Analyze does not return on it)");
+    if (T > 256) return fail(ctx, WVA_EINVAL, "the device greedy solver holds at most 256 accelerator types");
+    if ((unsigned long long)(S ? S : 1) * (unsigned long long)A >= (1ull << 31))
+        return fail(ctx, WVA_EINVAL, "servers x accelerators must stay below 2^31 for the greedy solver");
+    if (ctx->s0 != 0 || ctx->ns != S)
+        return fail(ctx, WVA_ESTATE, "wva_solve_loads sizes every server: the context's shard must hold them all");
+    CK(cudaSetDevice(ctx->device));
+    const int policy = spec->saturation_policy, dbe = spec->delayed_best_effort ? 1 : 0;
+    const size_t SA = (size_t)S * A;
+    GreedyPlan gp;
+    const size_t region = align_up(greedy_carve(ctx, nullptr, gp), 256);
+    const int path = S > 0 ? gp.path : 0;
+    const size_t smem = path == 3 ? greedy_scan_smem(gp, policy) : 0;
+    // per scenario: plane and slow-list entries, records (44 bytes of fields and a feasible byte per pair), rates, greedy
+    // buffers, outputs
+    const size_t perScen = SA * (sizeof(wva_pair_rec) + 8 + 45) + (size_t)S * 4 + (path ? region + sizeof(GreedyLoadView) : 0) +
+                           (size_t)S * (4 + sizeof(wva_pair_rec)) + (size_t)T * 12;
+    const size_t maxPerChunk = A > 0 ? 0x7fffffffULL / (size_t)A : (size_t)n_l;       // k_pairs_loads: A * nL < 2^31
+    const int nChunk = (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_l, ctx->sl_budget / perScen, maxPerChunk}));
+    const size_t nv1 = (size_t)nChunk, nvS = nv1 * S, nvSA = nv1 * SA;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
+    const size_t o_acc = take(nvSA * 4), o_rep = take(nvSA * 8), o_bat = take(nvSA * 8), o_cost = take(nvSA * 4), o_val = take(nvSA * 4),
+                 o_itl = take(nvSA * 4), o_ttft = take(nvSA * 4), o_rho = take(nvSA * 4), o_arr = take(nvSA * 4), o_fe = take(nvSA),
+                 o_reg = take(path ? nv1 * region : 0), o_view = take(nv1 * sizeof(GreedyLoadView)), o_oacc = take(nvS * 4),
+                 o_orec = take(nvS * sizeof(wva_pair_rec)), o_cnt = take(nv1 * T * 8), o_ocost = take(nv1 * T * 4), o_cyc = take(8);
+    CK(ctx->slChunk.ensure(off));
+    CK(ctx->plRpm.ensure((nvS ? nvS : 1) * 4));
+    CK(ctx->plPlane.ensure((nvSA ? nvSA : 1) * sizeof(wva_pair_rec)));
+    CK(ctx->plCount.ensure(64));
+    char* cb = ctx->slChunk.as<char>();
+    DevAllocs recs;
+    recs.acc = (int*)(cb + o_acc); recs.num_replicas = (long long*)(cb + o_rep); recs.batch_size = (long long*)(cb + o_bat);
+    recs.cost = (float*)(cb + o_cost); recs.value = (float*)(cb + o_val); recs.itl = (float*)(cb + o_itl); recs.ttft = (float*)(cb + o_ttft);
+    recs.rho = (float*)(cb + o_rho); recs.max_arrv = (float*)(cb + o_arr);
+    unsigned char* feas = (unsigned char*)(cb + o_fe);
+    GreedyLoadView* viewDev = (GreedyLoadView*)(cb + o_view);
+    int* accDev = (int*)(cb + o_oacc);
+    wva_pair_rec* recDev = (wva_pair_rec*)(cb + o_orec);
+    long long* cntDev = (long long*)(cb + o_cnt);
+    float* costDev = (float*)(cb + o_ocost);
+    unsigned long long* maxCyc = (unsigned long long*)(cb + o_cyc);
+    float* dRpm = ctx->plRpm.as<float>();
+    wva_pair_rec* dPlane = ctx->plPlane.as<wva_pair_rec>();
+    CK(cudaMemsetAsync(ctx->plCount.p, 0, 64, ctx->stream));
+    CK(cudaMemsetAsync(maxCyc, 0, 8, ctx->stream));
+    if (path == 3 && smem > 48 * 1024) CK(cudaFuncSetAttribute(k_greedy_scan_loads, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    std::vector<GreedyPlan> plans(nv1);
+    std::vector<GreedyLoadView> views(nv1);
+    uint64_t chunks = 0, nSlow = 0;
+    int rc = WVA_OK;
+    for (int j0 = 0; j0 < n_l; j0 += nChunk) {
+        const int nv = std::min(nChunk, n_l - j0);
+        const size_t n = (size_t)nv * S;
+        if (S > 0) {
+            CK(cudaMemcpy2DAsync(dRpm, (size_t)nv * 4, arrival_rpm + j0, (size_t)n_l * 4, (size_t)nv * 4, (size_t)S, cudaMemcpyHostToDevice,
+                                 ctx->stream));
+            rc = pairs_loads_run(ctx, 0, S, nv, dRpm, dPlane, nSlow);
+            if (rc != WVA_OK) return rc;
+            const size_t items = (size_t)nv * SA;
+            k_loads_records<<<(unsigned)((items + 255) / 256), 256, 0, ctx->stream>>>(dPlane, S, A, nv, recs, feas);
+            LAUNCH_CHECK();
+            for (int j = 0; j < nv; ++j) {
+                GreedyPlan& p = plans[(size_t)j];
+                greedy_carve(ctx, cb + o_reg + (size_t)j * region, p);
+                rc = greedy_order(ctx, p, allocs_at(recs, (size_t)j * SA), feas + (size_t)j * SA);
+                if (rc != WVA_OK) return rc;
+            }
+            if (path == 3) {
+                for (int j = 0; j < nv; ++j) {
+                    GreedyLoadView& v = views[(size_t)j];
+                    v.pairs = allocs_at(recs, (size_t)j * SA); v.g = plans[(size_t)j].g; v.g.smemBytes = (int)smem;
+                    v.gs = plans[(size_t)j].gsc; v.chosen = plans[(size_t)j].chosenKey;
+                }
+                CK(cudaMemcpyAsync(viewDev, views.data(), (size_t)nv * sizeof(GreedyLoadView), cudaMemcpyHostToDevice, ctx->stream));
+                k_greedy_scan_loads<<<nv, 32, smem, ctx->stream>>>(ctx->dsys, viewDev, dbe, policy, maxCyc);
+                LAUNCH_CHECK();
+            } else {
+                for (int j = 0; j < nv; ++j) {
+                    rc = greedy_launch(ctx, plans[(size_t)j], ctx->dsys, allocs_at(recs, (size_t)j * SA), dbe, policy);
+                    if (rc != WVA_OK) return rc;
+                }
+            }
+            for (int j = 0; j < nv; ++j) {
+                const GreedyPlan& p = plans[(size_t)j];
+                k_greedy_collect_multi<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, allocs_at(recs, (size_t)j * SA), p.g.order, p.chosenKey,
+                                                                              nullptr, nullptr, (size_t)S, accDev + (size_t)j * S,
+                                                                              recDev + (size_t)j * S);
+                LAUNCH_CHECK();
+            }
+        }
+        if (T > 0) {
+            k_totals_multi<<<dim3((unsigned)T, (unsigned)nv), 1024, 0, ctx->stream>>>(ctx->dsys, accDev, recDev, cntDev, costDev);
+            LAUNCH_CHECK();
+        }
+        if (chosen_acc && n) CK(cudaMemcpyAsync(chosen_acc + (size_t)j0 * S, accDev, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        if (chosen && n) CK(cudaMemcpyAsync(chosen + (size_t)j0 * S, recDev, n * sizeof(wva_pair_rec), cudaMemcpyDeviceToHost, ctx->stream));
+        if (type_count && T) CK(cudaMemcpyAsync(type_count + (size_t)j0 * T, cntDev, (size_t)nv * T * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        if (type_cost && T) CK(cudaMemcpyAsync(type_cost + (size_t)j0 * T, costDev, (size_t)nv * T * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));       // the next chunk reuses the chunk's buffers
+        ++chunks;
+    }
+    unsigned long long dev[6], cyc = 0;
+    CK(cudaMemcpy(dev, ctx->plCount.as<char>() + 8, sizeof dev, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&cyc, maxCyc, 8, cudaMemcpyDeviceToHost));
+    ctx->sl_counters[0] = chunks; ctx->sl_counters[1] = (uint64_t)path; ctx->sl_counters[2] = dev[4]; ctx->sl_counters[3] = dev[5];
+    ctx->sl_counters[4] = nSlow; ctx->sl_counters[5] = cyc;
+    return WVA_OK;
+}
+int wva_solve_loads_counters(const wva_ctx* ctx, uint64_t out[6]) {
+    if (!ctx || !out) return WVA_EINVAL;
+    for (int k = 0; k < 6; ++k) out[k] = ctx->sl_counters[k];
+    return WVA_OK;
+}
+int wva_solve_loads_set_budget(wva_ctx* ctx, int64_t bytes) {
+    if (!ctx || bytes < 0) return WVA_EINVAL;
+    ctx->sl_budget = bytes == 0 ? (size_t)1 << 28 : (size_t)bytes;
     return WVA_OK;
 }
 

@@ -440,4 +440,42 @@ __global__ void __launch_bounds__(1024) k_totals_multi(DevSystem sys, const int*
     totals_block(sys, blockIdx.x, 0, sys.S, TotalsPairRec{chosen_acc + j * sys.S, chosen + j * sys.S}, count + j * sys.T, cost + j * sys.T);
 }
 
+// ---- many arrival-rate scenarios (wva_solve_loads) ---------------------------------------------------------------
+// The candidate values depend on the load, so every scenario has records, a candidate order, a static order and greedy
+// buffers of its own (one GreedyPlan each, built by the kernels above); only the image, its capacities included, is
+// shared.  Each scenario's records are used once, so best effort scales them in place as in wva_solve.
+
+// chunk records, scenario-major: plane item ((s * nL + j) * A + a) of k_pairs_loads -> (j * S + s) * A + a, so that
+// scenario j's records are a DevAllocs at offset j * S * A
+__global__ void k_loads_records(const wva_pair_rec* __restrict__ plane, int S, int A, int nL, DevAllocs out, unsigned char* __restrict__ feasible) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)S * nL * A) return;
+    const size_t a = i % (size_t)A, sj = i / (size_t)A, j = sj % (size_t)nL, s = sj / (size_t)nL;
+    const size_t o = (j * S + s) * A + a;
+    const wva_pair_rec r = plane[i];
+    out.acc[o] = r.acc; out.num_replicas[o] = r.num_replicas; out.batch_size[o] = r.batch_size;
+    out.cost[o] = r.cost; out.value[o] = r.value; out.itl[o] = r.itl; out.ttft[o] = r.ttft; out.rho[o] = r.rho;
+    out.max_arrv[o] = r.max_arrv_rate_per_replica;
+    feasible[o] = r.feasible;
+}
+
+// what the pass of one scenario works on: its records, its greedy buffers, its static order and its chosen slots
+struct GreedyLoadView {
+    DevAllocs pairs; GreedyBufs g; GreedyScan gs; int* chosen;
+};
+
+// the static-order pass of k_greedy_scan once per scenario, one block of one warp each; maxCycles = SM cycles of the
+// slowest scenario's pass
+__global__ void __launch_bounds__(32) k_greedy_scan_loads(DevSystem sys, const GreedyLoadView* __restrict__ views, int delayedBestEffort,
+                                                            int policy, unsigned long long* maxCycles) {
+    extern __shared__ __align__(16) unsigned char greedy_pool[];
+    __shared__ long long avail[256];
+    __shared__ long long usum[256];
+    const GreedyLoadView& v = views[blockIdx.x];
+    GreedyCtx c; c.sys = sys; c.pairs = v.pairs; c.g = v.g; c.chosen = v.chosen; c.avail = avail; c.usum = usum; c.lane = threadIdx.x;
+    unsigned long long st[4];
+    greedy_scan_pass(c, v.gs, sys.type_capacity, greedy_pool, delayedBestEffort, policy, [](int g0) { return g0; }, st);
+    if (threadIdx.x == 0) atomicMax(maxCycles, st[2] + st[3]);
+}
+
 }  // namespace wva
