@@ -252,7 +252,11 @@ int wva_shard_info(const wva_ctx* ctx, int32_t* first, int32_t* count);
  * followed by value = curAllocation.TransitionPenalty(alloc) (:291-300).
  * out has S*A records (server-major); feasible[s*A+a] = 1 when CreateAllocation
  * returned non-nil and the accelerator is a candidate for the server.  Results stay
- * resident on the device for wva_solve.  out / feasible may be NULL (device only). */
+ * resident on the device for wva_solve.  out / feasible may be NULL (device only).
+ * A pair whose chain needs rescaling is re-run with p[] materialised in HBM (11 N + 1 doubles).  Such items run in
+ * chunks whose scratch fits the larger of half the free device memory and the scratch the context already holds;
+ * WVA_ECUDA only when one item alone does not fit.  The other pair calls and wva_queue_analyze / wva_queue_size
+ * follow the same rule. */
 int wva_analyze_pairs(wva_ctx* ctx, wva_alloc_soa* out, uint8_t* feasible);
 
 /* Candidate sweep (north_star): for every (server, accelerator, replicas r in 1..r_max,
@@ -398,8 +402,8 @@ int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]);
  *         record (acc = -1, feasible = 0) where it chooses none.
  * QueueAnalyzer.Size does not read the load, so it runs once per pair whatever n_l is.  The records are staged in HBM in
  * slices of at most 2^28 bytes of servers (one server at least): each slice's rows of arrival_rpm are copied in and its
- * records copied out before the next starts.  Items that need the materialised-p[] path run in chunks that fit half
- * the free device memory; WVA_ECUDA only when one item alone does not fit (where wva_analyze_pairs fails too).  Nothing that other calls read changes: pair records, decisions, totals,
+ * records copied out before the next starts.  Items that need the materialised-p[] path run in chunks, as in
+ * wva_analyze_pairs.  Nothing that other calls read changes: pair records, decisions, totals,
  * sweep results and the resident image (srv_arrival_rpm included), and whether they are valid, stay as they were.
  * WVA_EINVAL for n_l out of range, arrival_rpm == NULL while the shard has servers, or a NaN rate (the reference's
  * Analyze does not return on it); WVA_ESTATE before any upload.  Both change nothing. */

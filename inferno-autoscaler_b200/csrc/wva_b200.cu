@@ -4,6 +4,7 @@
 // implementation of any arithmetic in this file (and no fallback when CUDA is unavailable).
 #include "wva_kernels.cuh"
 #include "wva_block.cuh"
+#include "wva_scratch_plan.h"
 
 #include <algorithm>
 #include <atomic>
@@ -150,7 +151,8 @@ struct wva_ctx {
     // N from the uploaded image (pair_batch_size without the validity tests), offsets for the shard
     std::vector<long long> hostN;
     bool plan_valid = false;
-    long long plan_total = 0, plan_maxN = 0;
+    long long plan_maxN = 0;
+    int plan_smem = 0;
     cudaStream_t stream = nullptr;
     cudaStream_t gstream = nullptr;      // the candidate sweep has its own stream so it can overlap the pair sizing
     cudaStream_t gstream2 = nullptr;     // k_scan_lean runs beside k_scan_cert and the exact-chain kernels
@@ -188,11 +190,12 @@ struct wva_ctx {
     int grid_scan = 1;          // certified sweeps: 1 = the scan kernels k_scan_prep / k_scan_cert / k_scan_lean (default), 0 = the round-1 kernels
     int pairs_debug = 0;
     DevBuf pairDbg;
-    // wva_analyze_pairs_batches: buffers of its own, so the resident pair results above stay as they are
-    DevBuf pbBatch, pbSlow, pbScratch, pbScratchOff, pbPlane, pbBest, pbCount;
+    // wva_analyze_pairs_batches: buffers of its own, so the resident pair results above stay as they are (the
+    // materialised path runs in scratch / scratchOff, as every pair and queue call's does: see run_materialised)
+    DevBuf pbBatch, pbSlow, pbPlane, pbBest, pbCount;
     uint64_t pb_counters[4] = {0, 0, 0, 0};
     // wva_analyze_pairs_loads: likewise, with a table plan of its own
-    DevBuf plRpm, plSlow, plScratch, plScratchOff, plPlane, plBest, plCount, plTabOff, plTabs;
+    DevBuf plRpm, plSlow, plPlane, plBest, plCount, plTabOff, plTabs;
     uint64_t pl_counters[5] = {0, 0, 0, 0, 0};
 
     // solution
@@ -211,7 +214,7 @@ struct wva_ctx {
     DevBuf capShared, capSlots, capChunk, capPairs;
     size_t cap_budget = (size_t)1 << 28;
     uint64_t cap_counters[4] = {0, 0, 0, 0};
-    // wva_solve_loads: chunk buffer of its own (pair sizing runs in wva_analyze_pairs_loads's scratch), budget, counters
+    // wva_solve_loads: chunk buffer of its own (pair sizing runs in wva_analyze_pairs_loads's buffers), budget, counters
     DevBuf slChunk;
     size_t sl_budget = (size_t)1 << 28;
     uint64_t sl_counters[6] = {0, 0, 0, 0, 0, 0};
@@ -366,6 +369,62 @@ int comm_gather_pairs(wva_ctx* ctx) {
     return WVA_OK;
 }
 
+// The materialised-p[] path of the pair and queue calls: item i of a list re-runs its chain with p[] in a scratch row
+// of len[i] doubles.  The items run in list order, in chunks whose rows fit max(half the free device memory, the
+// scratch already held); launch(i0, n) starts the caller's literal kernel on items [i0, i0 + n) of its list, with
+// ctx->scratch and the chunk's row offsets in ctx->scratchOff.  WVA_ECUDA only when one item alone does not fit.
+// Returns with the stream drained.
+template <class Launch>
+int run_materialised(wva_ctx* ctx, const std::vector<long long>& len, Launch launch) {
+    size_t freeB = 0, totB = 0;
+    CK(cudaMemGetInfo(&freeB, &totB));
+    const long long capDoubles = (long long)(std::max(freeB / 2, ctx->scratch.cap) / 8);
+    std::vector<long long> offs;
+    for (size_t i0 = 0; i0 < len.size();) {
+        const ScratchChunk c = scratch_chunk(len, i0, capDoubles, offs);
+        if (c.end == i0) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
+        const size_t n = c.end - i0;
+        CK(ctx->scratch.ensure((size_t)c.doubles * 8));
+        CK(ctx->scratchOff.ensure(n * 8));
+        CK(cudaMemcpyAsync(ctx->scratchOff.p, offs.data(), n * 8, cudaMemcpyHostToDevice, ctx->stream));
+        launch(i0, (int)n);
+        LAUNCH_CHECK();
+        CK(cudaStreamSynchronize(ctx->stream));      // the next chunk reuses the scratch and its offsets
+        i0 = c.end;
+    }
+    return WVA_OK;
+}
+
+// The {rate, reciprocal} table plan of k_pairs_warp and k_pairs_loads, from the N of nPairs pairs.  A table that fits
+// the warp's shared-memory slice (up to 3072 entries, 48 KB; with pairs_smem) needs no HBM at all: only larger ones
+// draw on the 2 GB budget (round 1 reserved HBM for every pair; at 800 000 pairs per rank -- BASELINE config 5 -- that
+// blew the budget and sent most pairs to the materialised path).  tabOff[i] = -1 sends pair i to the materialised path
+// (above 2^26 entries or over the budget); 0 is unused (no queueing work, or a shared-memory table).  Uploads the
+// offsets and drains the stream (they are a local); maxN = the largest N up to 2^26, smemEntries = table entries per
+// warp in shared memory.
+int plan_pair_tables(wva_ctx* ctx, const long long* nPair, int nPairs, DevBuf& tabOff, DevBuf& tabs, long long& maxN,
+                     int& smemEntries) {
+    const long long budget = (2LL << 30) / 16;
+    maxN = 0;
+    for (int i = 0; i < nPairs; ++i) if (nPair[i] > maxN && nPair[i] <= (1LL << 26)) maxN = nPair[i];
+    smemEntries = ctx->pairs_smem ? (int)std::min(maxN, 3072LL) : 0;
+    std::vector<long long> offs((size_t)nPairs);
+    long long total = 0;
+    for (int i = 0; i < nPairs; ++i) {
+        const long long N = nPair[i];
+        if (N <= 0 || N <= smemEntries) { offs[(size_t)i] = 0; continue; }
+        if (N > (1LL << 26) || total + N > budget) { offs[(size_t)i] = -1; continue; }
+        offs[(size_t)i] = total; total += N;
+    }
+    CK(tabs.ensure((size_t)(total ? total : 1) * 16));
+    CK(tabOff.ensure((size_t)nPairs * 8));
+    CK(cudaMemcpyAsync(tabOff.p, offs.data(), (size_t)nPairs * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return WVA_OK;
+}
+// dynamic shared memory of a k_pairs_warp / k_pairs_loads block: smemEntries table entries per warp
+size_t pair_smem_bytes(int smemEntries) { return (size_t)smemEntries * 16 * (WVA_PAIRS_WARP_THREADS / 32); }
+
 }  // namespace
 
 extern "C" {
@@ -443,9 +502,8 @@ void wva_ctx_destroy(wva_ctx* ctx) {
                       &ctx->heavyOrder, &ctx->heavyHist, &ctx->pairTab, &ctx->blockSlot, &ctx->listSlot, &ctx->gscratch, &ctx->rowInfo, &ctx->rateTab, &ctx->ioA, &ctx->ioB,
                       &ctx->ioC, &ctx->ioD, &ctx->ioE, &ctx->ioF, &ctx->ioG, &ctx->commTotals, &ctx->commChunk, &ctx->commGather,
                       &ctx->blkPlane, &ctx->blkExact, &ctx->blkLit, &ctx->blkCount, &ctx->blkCounts, &ctx->blkScratch, &ctx->blkIo,
-                      &ctx->pbBatch, &ctx->pbSlow, &ctx->pbScratch, &ctx->pbScratchOff,
-                      &ctx->pbPlane, &ctx->pbBest, &ctx->pbCount,
-                      &ctx->plRpm, &ctx->plSlow, &ctx->plScratch, &ctx->plScratchOff, &ctx->plPlane, &ctx->plBest,
+                      &ctx->pbBatch, &ctx->pbSlow, &ctx->pbPlane, &ctx->pbBest, &ctx->pbCount,
+                      &ctx->plRpm, &ctx->plSlow, &ctx->plPlane, &ctx->plBest,
                       &ctx->plCount, &ctx->plTabOff, &ctx->plTabs, &ctx->slChunk};
     for (DevBuf* b : bufs) b->release();
     ctx->staging.release();
@@ -613,32 +671,15 @@ int wva_analyze_pairs(wva_ctx* ctx, wva_alloc_soa* out, uint8_t* feasible) {
             // latency-oriented variant: one warp per pair, per-pair {rate, reciprocal} tables in HBM; the table
             // plan comes from the host copy of N (made at upload) and is kept while image and shard stay
             if (!ctx->plan_valid) {
-                std::vector<long long> offs((size_t)nPairs);
-                long long total = 0, maxN = 0;
-                const long long budget = (2LL << 30) / 16;          // at most 2 GB of tables
-                const long long* nHost = ctx->hostN.data() + (size_t)ctx->s0 * A;
-                for (int i = 0; i < nPairs; ++i) { const long long N = nHost[(size_t)i]; if (N > maxN && N <= (1LL << 26)) maxN = N; }
-                // a pair whose table fits the warp's shared-memory slice (<= 3072 entries) needs no table in HBM at all: only
-                // larger ones draw on the budget (round 1 reserved HBM for every pair; at 800 000 pairs per rank -- BASELINE
-                // config 5 -- that blew the budget and sent most pairs to the materialised path)
-                const long long inSmem = ctx->pairs_smem ? (maxN < 3072 ? maxN : 3072) : 0;
-                for (int i = 0; i < nPairs; ++i) {
-                    long long N = nHost[(size_t)i];
-                    if (N <= 0 || N <= inSmem) { offs[(size_t)i] = 0; continue; }   // no queueing work, or table in shared memory: offset unused
-                    if (N > (1LL << 26) || total + N > budget) { offs[(size_t)i] = -1; continue; }
-                    offs[(size_t)i] = total; total += N;
-                }
-                CK(ctx->pairTabs.ensure((size_t)(total ? total : 1) * 16));
-                CK(ctx->pairTabOff.ensure((size_t)nPairs * 8));
-                CK(cudaMemcpyAsync(ctx->pairTabOff.p, offs.data(), (size_t)nPairs * 8, cudaMemcpyHostToDevice, ctx->stream));
-                CK(cudaStreamSynchronize(ctx->stream));               // offs is a local
-                ctx->plan_total = total; ctx->plan_maxN = maxN; ctx->plan_valid = true;
+                const int rc = plan_pair_tables(ctx, ctx->hostN.data() + (size_t)ctx->s0 * A, nPairs, ctx->pairTabOff, ctx->pairTabs,
+                                                ctx->plan_maxN, ctx->plan_smem);
+                if (rc != WVA_OK) return rc;
+                ctx->plan_valid = true;
             }
             const long long maxN = ctx->plan_maxN;
+            const int smemEntries = ctx->plan_smem;
             const int warpsPerBlock = WVA_PAIRS_WARP_THREADS / 32;
-            // shared-memory tables: up to 3072 entries (48 KB) per warp, 4 warps per block
-            int smemEntries = ctx->pairs_smem ? (int)(maxN < 3072 ? maxN : 3072) : 0;
-            const size_t smemBytes = (size_t)smemEntries * 16 * warpsPerBlock;
+            const size_t smemBytes = pair_smem_bytes(smemEntries);
             if (smemBytes > 48 * 1024)
                 CK(cudaFuncSetAttribute(k_pairs_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
             // chain-value buffers (pass 2 reads p[n] back instead of re-running the recurrence): one
@@ -698,25 +739,18 @@ int wva_analyze_pairs(wva_ctx* ctx, wva_alloc_soa* out, uint8_t* feasible) {
         LAUNCH_CHECK();
         CK(cudaMemcpyAsync(nAllPairs.data(), ctx->pairN.p, (size_t)nPairs * 8, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        std::vector<long long> offs((size_t)slow);
-        long long total = 0;
+        std::vector<long long> len((size_t)slow);
         for (int i = 0; i < slow; ++i) {
             long long N = nAllPairs[(size_t)list[(size_t)i]];
             if (N > (1LL << 32)) return fail(ctx, WVA_EINVAL, "pair needs the materialised path with an unreasonably large batch size");
-            offs[(size_t)i] = total;
-            total += 11 * N + 1;
+            len[(size_t)i] = 11 * N + 1;
         }
-        size_t freeB = 0, totB = 0;
-        CK(cudaMemGetInfo(&freeB, &totB));
-        if ((size_t)total * 8 > freeB / 2) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-        CK(ctx->scratch.ensure((size_t)total * 8));
-        CK(ctx->scratchOff.ensure((size_t)slow * 8));
-        CK(cudaMemcpyAsync(ctx->scratchOff.p, offs.data(), (size_t)slow * 8, cudaMemcpyHostToDevice, ctx->stream));
-        k_pairs_literal<<<(slow + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, ctx->s0, ctx->slowList.as<int>(), slow,
-                                                                 ctx->scratch.as<double>(), ctx->scratchOff.as<long long>(),
-                                                                 ctx->pairs, ctx->feasible, ctx->stepCounter.as<unsigned long long>());
-        LAUNCH_CHECK();
-        CK(cudaStreamSynchronize(ctx->stream));
+        const int rc = run_materialised(ctx, len, [&](size_t i0, int n) {
+            k_pairs_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, ctx->s0, ctx->slowList.as<int>() + i0, n,
+                                                                  ctx->scratch.as<double>(), ctx->scratchOff.as<long long>(),
+                                                                  ctx->pairs, ctx->feasible, ctx->stepCounter.as<unsigned long long>());
+        });
+        if (rc != WVA_OK) return rc;
     }
     timer.stop();
     ctx->pairs_valid = true;
@@ -839,7 +873,7 @@ int wva_analyze_pairs_batches(wva_ctx* ctx, int32_t n_b, const int32_t* batch, w
     const size_t smemBytes = (size_t)batch[n_b - 1] * 16;        // the table up to the largest b: at most 128 KB
     if (smemBytes > 48 * 1024) CK(cudaFuncSetAttribute(k_pairs_plane, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
     std::vector<unsigned long long> items;
-    std::vector<long long> offs;
+    std::vector<long long> len;
     uint64_t nSlices = 0, nSlow = 0;
     for (int f = ctx->s0; f < ctx->s0 + ns; f += slice) {
         const int nss = std::min(slice, ctx->s0 + ns - f);
@@ -854,19 +888,14 @@ int wva_analyze_pairs_batches(wva_ctx* ctx, int32_t n_b, const int32_t* batch, w
         if (slow > 0) {
             // items whose chain hit an overflow-rescale branch or whose table prefix holds an unusable entry: p[] in HBM
             items.resize((size_t)slow);
-            offs.resize((size_t)slow);
+            len.resize((size_t)slow);
             CK(cudaMemcpy(items.data(), dSlow, (size_t)slow * 8, cudaMemcpyDeviceToHost));
-            long long total = 0;
-            for (int i = 0; i < slow; ++i) { offs[(size_t)i] = total; total += 11LL * batch[items[(size_t)i] % (unsigned)n_b] + 1; }
-            size_t freeB = 0, totB = 0;
-            CK(cudaMemGetInfo(&freeB, &totB));
-            if ((size_t)total * 8 > freeB / 2) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-            CK(ctx->pbScratch.ensure((size_t)total * 8));
-            CK(ctx->pbScratchOff.ensure((size_t)slow * 8));
-            CK(cudaMemcpyAsync(ctx->pbScratchOff.p, offs.data(), (size_t)slow * 8, cudaMemcpyHostToDevice, ctx->stream));
-            k_pairs_plane_literal<<<(slow + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, dBatch, n_b, dSlow, slow, ctx->pbScratch.as<double>(),
-                                                                           ctx->pbScratchOff.as<long long>(), dPlane, counters);
-            LAUNCH_CHECK();
+            for (int i = 0; i < slow; ++i) len[(size_t)i] = 11LL * batch[items[(size_t)i] % (unsigned)n_b] + 1;
+            const int rc = run_materialised(ctx, len, [&](size_t i0, int n) {
+                k_pairs_plane_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, dBatch, n_b, dSlow + i0, n, ctx->scratch.as<double>(),
+                                                                            ctx->scratchOff.as<long long>(), dPlane, counters);
+            });
+            if (rc != WVA_OK) return rc;
             nSlow += (uint64_t)slow;
         }
         k_pairs_plane_best<<<(nss + 3) / 4, 128, 0, ctx->stream>>>(dPlane, nss, (int)perServer, dBest);
@@ -874,7 +903,7 @@ int wva_analyze_pairs_batches(wva_ctx* ctx, int32_t n_b, const int32_t* batch, w
         const size_t hs = (size_t)(f - ctx->s0);
         if (plane) CK(cudaMemcpyAsync(plane + hs * perServer, dPlane, (size_t)nss * recBytes, cudaMemcpyDeviceToHost, ctx->stream));
         if (best) CK(cudaMemcpyAsync(best + hs, dBest, (size_t)nss * sizeof(wva_pair_rec), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));       // also releases offs for the next slice
+        CK(cudaStreamSynchronize(ctx->stream));       // the next slice reuses the slice's buffers
         ++nSlices;
     }
     unsigned long long dev[5];
@@ -897,45 +926,26 @@ int wva_pairs_batches_counters(const wva_ctx* ctx, uint64_t out[4]) {
 // Pair sizing of servers [f, f + nss) under nL scenarios: the rates are on the device already, rpm[(s - f) * nL + j], and
 // record (s, j, a) lands at plane[((s - f) * nL + j) * A + a].  The rate tables are planned here from N under a positive
 // load (the plan of wva_analyze_pairs follows the uploaded rates and gives a zero-load server no table); k_pairs_loads
-// sizes each pair once and k_pairs_loads_literal re-runs the items it sent to the materialised path.  Scratch and
+// sizes each pair once and k_pairs_loads_literal re-runs the items it sent to the materialised path.  Tables and
 // counters are wva_analyze_pairs_loads's (ctx->plCount: [0, 4) slow-list length, [8, 56) k_pairs_loads's counters,
 // zeroed by the caller); nSlow grows by the items of the materialised path.  Returns with the stream drained.
 static int pairs_loads_run(wva_ctx* ctx, int f, int nss, int n_l, const float* dRpm, wva_pair_rec* dPlane, uint64_t& nSlow) {
     const int A = ctx->A;
     CK(ctx->plSlow.ensure((size_t)nss * A * n_l * 8));
-    CK(ctx->plTabOff.ensure((size_t)nss * A * 8));
     char* cnt = ctx->plCount.as<char>();
     int* slowCount = reinterpret_cast<int*>(cnt);
     unsigned long long* counters = reinterpret_cast<unsigned long long*>(cnt + 8);
     unsigned long long* dSlow = ctx->plSlow.as<unsigned long long>();
     const int warpsPerBlock = WVA_PAIRS_WARP_THREADS / 32;
-    const long long budget = (2LL << 30) / 16;           // at most 2 GB of tables, as wva_analyze_pairs
-    std::vector<long long> nPair, offs;
-    std::vector<unsigned long long> items;
-    std::vector<long long> soffs;
     const int nPairs = nss * A;
-    // table plan: the warp's shared-memory slice up to 3072 entries, HBM above that under the budget, the
-    // materialised path beyond it or above 2^26 entries
-    nPair.resize((size_t)nPairs);
-    offs.resize((size_t)nPairs);
-    long long maxN = 0, total = 0;
-    for (int i = 0; i < nPairs; ++i) {
-        const long long N = host_pair_n(ctx, f + i / A, i % A);
-        nPair[(size_t)i] = N;
-        if (N > maxN && N <= (1LL << 26)) maxN = N;
-    }
-    const long long inSmem = ctx->pairs_smem ? (maxN < 3072 ? maxN : 3072) : 0;
-    for (int i = 0; i < nPairs; ++i) {
-        const long long N = nPair[(size_t)i];
-        if (N <= 0 || N <= inSmem) { offs[(size_t)i] = 0; continue; }
-        if (N > (1LL << 26) || total + N > budget) { offs[(size_t)i] = -1; continue; }
-        offs[(size_t)i] = total; total += N;
-    }
-    CK(ctx->plTabs.ensure((size_t)(total ? total : 1) * 16));
-    CK(cudaMemcpyAsync(ctx->plTabOff.p, offs.data(), (size_t)nPairs * 8, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<long long> nPair((size_t)nPairs);
+    for (int i = 0; i < nPairs; ++i) nPair[(size_t)i] = host_pair_n(ctx, f + i / A, i % A);
+    long long maxN = 0;
+    int smemEntries = 0;
+    int rc = plan_pair_tables(ctx, nPair.data(), nPairs, ctx->plTabOff, ctx->plTabs, maxN, smemEntries);
+    if (rc != WVA_OK) return rc;
     CK(cudaMemsetAsync(slowCount, 0, 4, ctx->stream));
-    const int smemEntries = (int)inSmem;
-    const size_t smemBytes = (size_t)smemEntries * 16 * warpsPerBlock;
+    const size_t smemBytes = pair_smem_bytes(smemEntries);
     if (smemBytes > 48 * 1024) CK(cudaFuncSetAttribute(k_pairs_loads, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
     k_pairs_loads<<<(nPairs + warpsPerBlock - 1) / warpsPerBlock, WVA_PAIRS_WARP_THREADS, smemBytes, ctx->stream>>>(
         ctx->dsys, f, nPairs, n_l, dRpm, ctx->plTabOff.as<long long>(), ctx->plTabs.as<double2>(), smemEntries, dPlane, dSlow,
@@ -945,36 +955,22 @@ static int pairs_loads_run(wva_ctx* ctx, int f, int nss, int n_l, const float* d
     CK(cudaMemcpyAsync(&slow, slowCount, 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (slow > 0) {
-        // items whose chain hit an overflow-rescale branch, or whose pair has no usable table: p[] in HBM.  A pair
-        // can send all n_l of its items here, so they run in chunks whose scratch fits half the free memory: the call
-        // fails only when a single item does not fit, where wva_analyze_pairs fails too.
-        items.resize((size_t)slow);
-        soffs.resize((size_t)slow);
+        // items whose chain hit an overflow-rescale branch, or whose pair has no usable table: p[] in HBM (a pair can
+        // send all n_l of its items here)
+        std::vector<unsigned long long> items((size_t)slow);
+        std::vector<long long> len((size_t)slow);
         CK(cudaMemcpy(items.data(), dSlow, (size_t)slow * 8, cudaMemcpyDeviceToHost));
-        size_t freeB = 0, totB = 0;
-        CK(cudaMemGetInfo(&freeB, &totB));
-        const size_t capB = std::max(freeB / 2, ctx->plScratch.cap);
-        for (int i0 = 0; i0 < slow;) {
-            long long stotal = 0;
-            int i1 = i0;
-            for (; i1 < slow; ++i1) {
-                const unsigned long long it = items[(size_t)i1];
-                const long long N = nPair[(size_t)((it / (unsigned long long)A) / (unsigned long long)n_l * A + it % (unsigned long long)A)];
-                if (N > (1LL << 32)) return fail(ctx, WVA_EINVAL, "pair needs the materialised path with an unreasonably large batch size");
-                if (i1 > i0 && (size_t)(stotal + 11 * N + 1) * 8 > capB) break;
-                soffs[(size_t)(i1 - i0)] = stotal; stotal += 11 * N + 1;
-            }
-            if ((size_t)stotal * 8 > capB) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-            const int n = i1 - i0;
-            CK(ctx->plScratch.ensure((size_t)stotal * 8));
-            CK(ctx->plScratchOff.ensure((size_t)n * 8));
-            CK(cudaMemcpyAsync(ctx->plScratchOff.p, soffs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-            k_pairs_loads_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, n_l, dRpm, dSlow + i0, n, ctx->plScratch.as<double>(),
-                                                                        ctx->plScratchOff.as<long long>(), dPlane, counters);
-            LAUNCH_CHECK();
-            CK(cudaStreamSynchronize(ctx->stream));      // the next chunk reuses the scratch and its offsets
-            i0 = i1;
+        for (int i = 0; i < slow; ++i) {
+            const unsigned long long it = items[(size_t)i];
+            const long long N = nPair[(size_t)((it / (unsigned long long)A) / (unsigned long long)n_l * A + it % (unsigned long long)A)];
+            if (N > (1LL << 32)) return fail(ctx, WVA_EINVAL, "pair needs the materialised path with an unreasonably large batch size");
+            len[(size_t)i] = 11 * N + 1;
         }
+        rc = run_materialised(ctx, len, [&](size_t i0, int n) {
+            k_pairs_loads_literal<<<(n + 63) / 64, 64, 0, ctx->stream>>>(ctx->dsys, f, n_l, dRpm, dSlow + i0, n, ctx->scratch.as<double>(),
+                                                                        ctx->scratchOff.as<long long>(), dPlane, counters);
+        });
+        if (rc != WVA_OK) return rc;
         nSlow += (uint64_t)slow;
     }
     return WVA_OK;
@@ -2342,21 +2338,11 @@ int wva_type_totals_merge(wva_ctx* ctx, const void* gathered_dev, int32_t n_rank
 
 // ---------------------------------------------------------------------------------------------
 // low-level analyzer API
-static int queue_scratch(wva_ctx* ctx, const wva_queue_config* cfg, const std::vector<int>& list, DevBuf& offBuf) {
-    std::vector<long long> offs(list.size());
-    long long total = 0;
-    for (size_t i = 0; i < list.size(); ++i) {
-        const wva_queue_config& c = cfg[list[i]];
-        offs[i] = total;
-        total += (long long)c.max_batch_size + (long long)c.max_queue_size + 1;
-    }
-    size_t freeB = 0, totB = 0;
-    CK(cudaMemGetInfo(&freeB, &totB));
-    if ((size_t)total * 8 > freeB / 2) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-    CK(ctx->scratch.ensure((size_t)total * 8));
-    CK(offBuf.ensure(list.size() * 8));
-    CK(cudaMemcpyAsync(offBuf.p, offs.data(), list.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-    return WVA_OK;
+// scratch row of a queue item on the materialised path (the chain's K + 1 states)
+static std::vector<long long> queue_chain_len(const wva_queue_config* cfg, const std::vector<int>& list) {
+    std::vector<long long> len(list.size());
+    for (size_t i = 0; i < list.size(); ++i) len[i] = (long long)cfg[list[i]].max_batch_size + (long long)cfg[list[i]].max_queue_size + 1;
+    return len;
 }
 
 int wva_queue_analyze(wva_ctx* ctx, int32_t n, const wva_queue_config* cfg, const float* rate, wva_metrics* metrics, uint8_t* status) {
@@ -2382,15 +2368,15 @@ int wva_queue_analyze(wva_ctx* ctx, int32_t n, const wva_queue_config* cfg, cons
     if (nf > 0) {
         std::vector<int> list((size_t)nf);
         CK(cudaMemcpy(list.data(), ctx->faultList.p, (size_t)nf * 4, cudaMemcpyDeviceToHost));
-        int rc = queue_scratch(ctx, cfg, list, ctx->scratchOff);
-        if (rc != WVA_OK) return rc;
         CK(ctx->ioG.ensure((size_t)nf * 4));
         CK(cudaMemcpyAsync(ctx->ioG.p, list.data(), (size_t)nf * 4, cudaMemcpyHostToDevice, ctx->stream));
-        k_queue_analyze<<<(nf + 127) / 128, 128, 0, ctx->stream>>>(nf, ctx->ioA.as<wva_queue_config>(), ctx->ioB.as<float>(),
-                                                                  ctx->ioC.as<wva_metrics>(), ctx->ioD.as<unsigned char>(),
-                                                                  ctx->scratch.as<double>(), ctx->scratchOff.as<long long>(),
-                                                                  ctx->ioG.as<int>(), ctx->faultList.as<int>(), ctx->faultCount.as<int>());
-        LAUNCH_CHECK();
+        const int rc = run_materialised(ctx, queue_chain_len(cfg, list), [&](size_t i0, int m) {
+            k_queue_analyze<<<(m + 127) / 128, 128, 0, ctx->stream>>>(m, ctx->ioA.as<wva_queue_config>(), ctx->ioB.as<float>(),
+                                                                     ctx->ioC.as<wva_metrics>(), ctx->ioD.as<unsigned char>(),
+                                                                     ctx->scratch.as<double>(), ctx->scratchOff.as<long long>(),
+                                                                     ctx->ioG.as<int>() + i0, ctx->faultList.as<int>(), ctx->faultCount.as<int>());
+        });
+        if (rc != WVA_OK) return rc;
     }
     CK(cudaMemcpyAsync(metrics, ctx->ioC.p, (size_t)n * sizeof(wva_metrics), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(status, ctx->ioD.p, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2424,15 +2410,15 @@ int wva_queue_size(wva_ctx* ctx, int32_t n, const wva_queue_config* cfg, const f
     if (nf > 0) {
         std::vector<int> list((size_t)nf);
         CK(cudaMemcpy(list.data(), ctx->faultList.p, (size_t)nf * 4, cudaMemcpyDeviceToHost));
-        int rc = queue_scratch(ctx, cfg, list, ctx->scratchOff);
-        if (rc != WVA_OK) return rc;
         CK(ctx->ioG.ensure((size_t)nf * 4));
         CK(cudaMemcpyAsync(ctx->ioG.p, list.data(), (size_t)nf * 4, cudaMemcpyHostToDevice, ctx->stream));
-        k_queue_size<<<(nf + 127) / 128, 128, 0, ctx->stream>>>(nf, ctx->ioA.as<wva_queue_config>(), ctx->ioB.as<float>(), ctx->ioE.as<float>(),
-                                                               ctx->ioC.as<wva_metrics>(), ctx->ioF.as<float>(), ctx->ioD.as<unsigned char>(),
-                                                               ctx->scratch.as<double>(), ctx->scratchOff.as<long long>(), ctx->ioG.as<int>(),
-                                                               ctx->faultList.as<int>(), ctx->faultCount.as<int>());
-        LAUNCH_CHECK();
+        const int rc = run_materialised(ctx, queue_chain_len(cfg, list), [&](size_t i0, int m) {
+            k_queue_size<<<(m + 127) / 128, 128, 0, ctx->stream>>>(m, ctx->ioA.as<wva_queue_config>(), ctx->ioB.as<float>(), ctx->ioE.as<float>(),
+                                                                  ctx->ioC.as<wva_metrics>(), ctx->ioF.as<float>(), ctx->ioD.as<unsigned char>(),
+                                                                  ctx->scratch.as<double>(), ctx->scratchOff.as<long long>(), ctx->ioG.as<int>() + i0,
+                                                                  ctx->faultList.as<int>(), ctx->faultCount.as<int>());
+        });
+        if (rc != WVA_OK) return rc;
     }
     CK(cudaMemcpyAsync(rates, ctx->ioE.p, (size_t)n * 12, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(achieved, ctx->ioF.p, (size_t)n * 12, cudaMemcpyDeviceToHost, ctx->stream));

@@ -541,6 +541,26 @@ __device__ __forceinline__ void size_pair_warp(const DevSystem& sys, int s, int 
 }
 
 #define WVA_PAIRS_WARP_THREADS 128
+
+// BuildModel (queueanalyzer.go:99-131): pair pid's {rate, reciprocal} table of N entries, built by the warp's 32 lanes
+// together in the warp's shared-memory slice when it fits (29-cycle loads in the ramp), else at tabs + off in HBM.
+// nullptr when the pair has no table (off < 0 or N above 2^26: the host plan sends it to the materialised path) or an
+// entry is unusable.  The lane's chain values go to its column of pair pid's block of pbuf while the chain fits it.
+__device__ __forceinline__ double2* build_pair_table(WarpPair& wp, long long N, long long off, double2* smem, int smemEntriesPerWarp,
+                                                     double2* tabs, double* pbuf, long long pbufStrideK, int pid, int lane) {
+    if (off < 0 || N > (1LL << 26)) return nullptr;
+    double2* tab = (wp.N <= smemEntriesPerWarp) ? smem + (size_t)(threadIdx.x >> 5) * smemEntriesPerWarp : tabs + off;
+    wp.pstore = (pbuf && (long long)wp.K + 1 <= pbufStrideK) ? pbuf + (size_t)pid * (size_t)pbufStrideK * 32 + lane : nullptr;
+    bool bad = false;
+    for (int i = lane; i < wp.N; i += 32) {
+        const float r = wp.sv.rate(i + 1);
+        if (!(r > 0.0f) || !(r < CUDART_INF_F)) bad = true;
+        const double d = (double)r;
+        tab[i] = make_double2(d, rcp_refined(d));
+    }
+    __syncwarp();
+    return __any_sync(0xffffffffu, bad) ? nullptr : tab;
+}
 __global__ void __launch_bounds__(WVA_PAIRS_WARP_THREADS)
 k_pairs_warp(DevSystem sys, int s0, int nPairs, const long long* __restrict__ tabOff, double2* tabs, DevAllocs out,
              unsigned char* feasible, int* slow_list, int* slow_count, unsigned long long* step_counter,
@@ -560,22 +580,8 @@ k_pairs_warp(DevSystem sys, int s0, int nPairs, const long long* __restrict__ ta
     bool toSlow = false;      // needs the materialised path (whole pair re-done by k_pairs_literal)
 
     auto table = [&](WarpPair& wp, long long N) -> double2* {
-        if (tabOff[pid] < 0 || N > (1LL << 26)) return nullptr;   // no table budget: thread kernel handles it
-        // the table lives in shared memory when it fits (29-cycle loads in the ramp), else in HBM
-        double2* tab = (wp.N <= smemEntriesPerWarp)
-                           ? reinterpret_cast<double2*>(pairs_smem) + (size_t)(threadIdx.x >> 5) * smemEntriesPerWarp
-                           : tabs + tabOff[pid];
-        wp.pstore = (pbuf && (long long)wp.K + 1 <= pbufStrideK) ? pbuf + (size_t)pid * (size_t)pbufStrideK * 32 + lane : nullptr;
-        // BuildModel (queueanalyzer.go:99-131): the table, cooperatively
-        bool bad = false;
-        for (int i = lane; i < wp.N; i += 32) {
-            float r = wp.sv.rate(i + 1);
-            if (!(r > 0.0f) || !(r < CUDART_INF_F)) bad = true;
-            double d = (double)r;
-            tab[i] = make_double2(d, rcp_refined(d));
-        }
-        __syncwarp();
-        return __any_sync(0xffffffffu, bad) ? nullptr : tab;
+        return build_pair_table(wp, N, tabOff[pid], reinterpret_cast<double2*>(pairs_smem), smemEntriesPerWarp, tabs, pbuf, pbufStrideK,
+                                pid, lane);
     };
     size_pair_warp(sys, s, a, sys.srv_max_batch[s], table, lane, step_counter, rec, ok, toSlow, steps, activeRounds, totalRounds,
                    pendEvals, solveCycles);
@@ -886,20 +892,8 @@ k_pairs_loads(DevSystem sys, int s0, int nPairs, int nL, const float* __restrict
         if (config_ok(N, go_muli(N, WVA_MAX_QUEUE_TO_BATCH_RATIO), inTok, Kt)) {
             if (lane == 0) atomicAdd(counters + 4, 1ull);
             auto table = [&](WarpPair& w, long long n) -> double2* {
-                if (tabOff[pid] < 0 || n > (1LL << 26)) return nullptr;
-                double2* tab = (w.N <= smemEntriesPerWarp)
-                                   ? reinterpret_cast<double2*>(loads_smem) + (size_t)(threadIdx.x >> 5) * smemEntriesPerWarp
-                                   : tabs + tabOff[pid];
-                w.pstore = nullptr;
-                bool bad = false;
-                for (int i = lane; i < w.N; i += 32) {       // BuildModel (queueanalyzer.go:99-131)
-                    const float r = w.sv.rate(i + 1);
-                    if (!(r > 0.0f) || !(r < CUDART_INF_F)) bad = true;
-                    const double d = (double)r;
-                    tab[i] = make_double2(d, rcp_refined(d));
-                }
-                __syncwarp();
-                return __any_sync(0xffffffffu, bad) ? nullptr : tab;
+                return build_pair_table(w, n, tabOff[pid], reinterpret_cast<double2*>(loads_smem), smemEntriesPerWarp, tabs, nullptr, 0,
+                                        pid, lane);
             };
             auto atLambda = [&](const WarpPair& wp, const SolveStats& st, float lastX, float requestRate, long long n) {
                 // rateStar = Analyze(requestRate).Throughput (:237-241), from a lane's evaluation at that lambda if any
