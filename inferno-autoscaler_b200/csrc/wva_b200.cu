@@ -378,7 +378,7 @@ template <class Launch>
 int run_materialised(wva_ctx* ctx, const std::vector<long long>& len, Launch launch) {
     size_t freeB = 0, totB = 0;
     CK(cudaMemGetInfo(&freeB, &totB));
-    const long long capDoubles = (long long)(std::max(freeB / 2, ctx->scratch.cap) / 8);
+    const long long capDoubles = scratch_cap_doubles(freeB, ctx->scratch.cap);
     std::vector<long long> offs;
     for (size_t i0 = 0; i0 < len.size();) {
         const ScratchChunk c = scratch_chunk(len, i0, capDoubles, offs);
@@ -390,6 +390,25 @@ int run_materialised(wva_ctx* ctx, const std::vector<long long>& len, Launch lau
         launch(i0, (int)n);
         LAUNCH_CHECK();
         CK(cudaStreamSynchronize(ctx->stream));      // the next chunk reuses the scratch and its offsets
+        i0 = c.end;
+    }
+    return WVA_OK;
+}
+
+// The same rule for the sweep's and the blocking plane's lists, whose p[] rows all have `stride` doubles, in the caller's
+// buffer (they run beside pair sizing, so they cannot share ctx->scratch): launch(i0, n) starts the caller's literal
+// kernel on items [i0, i0 + n) with item i0 + k's row at k * stride.  The chunks follow each other on the caller's stream.
+template <class Launch>
+int run_materialised_rows(wva_ctx* ctx, size_t n, long long stride, DevBuf& buf, Launch launch) {
+    size_t freeB = 0, totB = 0;
+    CK(cudaMemGetInfo(&freeB, &totB));
+    const long long capDoubles = scratch_cap_doubles(freeB, buf.cap);
+    for (size_t i0 = 0; i0 < n;) {
+        const ScratchChunk c = scratch_chunk_rows(n, i0, stride, capDoubles);
+        if (c.end == i0) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
+        CK(buf.ensure((size_t)c.doubles * 8));
+        launch(i0, (int)(c.end - i0));
+        LAUNCH_CHECK();
         i0 = c.end;
     }
     return WVA_OK;
@@ -1157,13 +1176,14 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
         gp.r_chunk = (gp.r_chunk + WVA_SCAN_WARPS - 1) / WVA_SCAN_WARPS * WVA_SCAN_WARPS;
         gp.n_rchunks = (r_max + gp.r_chunk - 1) / gp.r_chunk;
     }
+    // k_scan_cert built for 3 resident blocks per SM (default) or 2 (wva_set_certified_tails bit 5)
+    void (*const scanCert)(DevSystem, GridParams) = ctx->grid_scan == 2 ? k_scan_cert<2> : k_scan_cert<3>;
     const size_t smem = (size_t)b_max * 20;
     if (smem > 48 * 1024) {
         CK(cudaFuncSetAttribute(k_grid, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CK(cudaFuncSetAttribute(k_grid_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CK(cudaFuncSetAttribute(k_scan_prep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CK(cudaFuncSetAttribute(k_scan_cert<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CK(cudaFuncSetAttribute(k_scan_cert<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(cudaFuncSetAttribute(scanCert, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     CK(cudaFuncSetAttribute(k_grid_list_own, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     // k_grid_wrow: the table, then per warp the checkpoints and the quotient buffer of warp_exact.  Only set when it
@@ -1181,6 +1201,19 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
     gp.rate_tab = scanMode ? ctx->rateTab.as<float2>() : nullptr;
     gp.block_slot = ctx->blockSlot.as<GridSlot>();
     const long long stride = 11LL * b_max + 1;
+    // the deferred list in ctx->heavyOrder, longest chain first: the first min(*gp.heavy_count, cap) entries, a count the
+    // kernels read from device memory, so both flows launch the same fixed grids
+    auto order_heavy = [&](int cap) -> int {
+        int* hist = ctx->heavyHist.as<int>();
+        CK(cudaMemsetAsync(hist, 0, 256 * 4, ctx->gstream));
+        k_heavy_hist<<<2 * ctx->num_sms, 256, 0, ctx->gstream>>>(gp.heavy_cost, gp.heavy_count, cap, hist);
+        LAUNCH_CHECK();
+        k_heavy_prefix<<<1, 256, 0, ctx->gstream>>>(hist);
+        LAUNCH_CHECK();
+        k_heavy_scatter<<<2 * ctx->num_sms, 256, 0, ctx->gstream>>>(gp.heavy_cost, gp.heavy_count, cap, hist, ctx->heavyOrder.as<int>());
+        LAUNCH_CHECK();
+        return WVA_OK;
+    };
 
     // order the sweep after whatever the main stream has queued (the system upload), run it on its own stream
     if (fork_join) {
@@ -1226,20 +1259,12 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
                 gp.list_slot = ctx->listSlot.as<GridSlot>();
                 k_scan_prep<<<(unsigned)nBlocks, WVA_SCAN_MAXROWS, smem, ctx->gstream>>>(ctx->dsys, gp);
                 LAUNCH_CHECK();
-                if (ctx->grid_scan == 2) k_scan_cert<2><<<(unsigned)nBlocks, WVA_SCAN_WARPS * 32, smem, ctx->gstream>>>(ctx->dsys, gp);
-                else k_scan_cert<3><<<(unsigned)nBlocks, WVA_SCAN_WARPS * 32, smem, ctx->gstream>>>(ctx->dsys, gp);
+                scanCert<<<(unsigned)nBlocks, WVA_SCAN_WARPS * 32, smem, ctx->gstream>>>(ctx->dsys, gp);
                 LAUNCH_CHECK();
                 ctx->sweep_launched.store(true, std::memory_order_release);
                 CK(cudaEventRecord(ctx->evk1, ctx->gstream));
                 CK(cudaEventRecord(ctx->evh0, ctx->gstream));
-                int* hist = ctx->heavyHist.as<int>();
-                CK(cudaMemsetAsync(hist, 0, 256 * 4, ctx->gstream));
-                k_heavy_hist_dev<<<2 * ctx->num_sms, 256, 0, ctx->gstream>>>(gp.heavy_cost, gp.heavy_count, (int)fusedCap, hist);
-                LAUNCH_CHECK();
-                k_heavy_prefix<<<1, 256, 0, ctx->gstream>>>(hist);
-                LAUNCH_CHECK();
-                k_heavy_scatter_dev<<<2 * ctx->num_sms, 256, 0, ctx->gstream>>>(gp.heavy_cost, gp.heavy_count, (int)fusedCap, hist, ctx->heavyOrder.as<int>());
-                LAUNCH_CHECK();
+                if (const int rc = order_heavy((int)fusedCap); rc != WVA_OK) return rc;
                 // both halves become runnable here; this stream has the higher priority, so the chain kernel's blocks are placed first
                 CK(cudaEventRecord(ctx->evPrep, ctx->gstream));
                 CK(cudaStreamWaitEvent(ctx->gstream2, ctx->evPrep, 0));
@@ -1282,8 +1307,7 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
                 // stream BESIDE the exact-chain kernels that follow on this one: those are a few hundred latency-bound warps,
                 // k_scan_lean is bound by the cube's HBM write.  (k_scan_lean asks for 46 KB of shared memory it does not use so
                 // that at most 4 of its blocks sit on an SM and a block of the exact-chain kernel still finds registers there.)
-                if (ctx->grid_scan == 2) k_scan_cert<2><<<(unsigned)nBlocks, WVA_SCAN_WARPS * 32, smem, ctx->gstream>>>(ctx->dsys, gp);
-                else k_scan_cert<3><<<(unsigned)nBlocks, WVA_SCAN_WARPS * 32, smem, ctx->gstream>>>(ctx->dsys, gp);
+                scanCert<<<(unsigned)nBlocks, WVA_SCAN_WARPS * 32, smem, ctx->gstream>>>(ctx->dsys, gp);
                 LAUNCH_CHECK();
                 CK(cudaEventRecord(ctx->evPrep, ctx->gstream));
                 CK(cudaStreamWaitEvent(ctx->gstream2, ctx->evPrep, 0));
@@ -1309,19 +1333,12 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
             gp.list_slot = ctx->listSlot.as<GridSlot>();
             if (heavy > 0) {
                 // long chains: order by estimated length (longest first), one thread per chain
-                int* hist = ctx->heavyHist.as<int>();
                 CK(cudaEventRecord(ctx->evh0, ctx->gstream));
                 const int* order = nullptr;
                 if (heavy >= 4096) {     // a short list fits in one wave: ordering it buys nothing.  Longer ones: the lanes of a warp
                                          // should hold chains of similar length (the warp lasts as long as its longest chain, and
                                          // solve_uni enters a block run only when every lane can)
-                    CK(cudaMemsetAsync(hist, 0, 256 * 4, ctx->gstream));
-                    k_heavy_hist<<<(heavy + 255) / 256, 256, 0, ctx->gstream>>>(gp.heavy_cost, heavy, hist);
-                    LAUNCH_CHECK();
-                    k_heavy_prefix<<<1, 256, 0, ctx->gstream>>>(hist);
-                    LAUNCH_CHECK();
-                    k_heavy_scatter<<<(heavy + 255) / 256, 256, 0, ctx->gstream>>>(gp.heavy_cost, heavy, hist, ctx->heavyOrder.as<int>());
-                    LAUNCH_CHECK();
+                    if (const int rc = order_heavy(heavy_cap); rc != WVA_OK) return rc;
                     order = ctx->heavyOrder.as<int>();
                 }
                 // few chains: the phase lasts as long as ONE exact chain -- one warp per chain (cooperative pass 2);
@@ -1354,20 +1371,11 @@ static int grid_run(wva_ctx* ctx, int r_max, int b_max, bool want_cube, bool wan
         ctx->last_heavy += heavy; ctx->last_slow += slow; ctx->last_heavy_slice = heavy; ctx->heavy_hint = heavy; ctx->last_fused = fused ? 1 : 0;
         int listSlots = heavy;
         if (slow > 0) {
-            size_t freeB = 0, totB = 0;
-            CK(cudaMemGetInfo(&freeB, &totB));
-            // process the literal list in pieces that fit in memory
-            size_t per = (size_t)stride * 8;
-            size_t maxItems = (freeB / 2) / per;
-            if (maxItems == 0) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-            if (maxItems > (size_t)slow) maxItems = (size_t)slow;
-            CK(ctx->gscratch.ensure(maxItems * per));
-            for (size_t done = 0; done < (size_t)slow; done += maxItems) {
-                int n = (int)(((size_t)slow - done) < maxItems ? ((size_t)slow - done) : maxItems);
-                k_grid_list<<<(n + 127) / 128, 128, 0, ctx->gstream>>>(ctx->dsys, gp, ctx->gridSlow.as<unsigned long long>() + done, nullptr,
-                                                                   n, ctx->gscratch.as<double>(), stride, heavy + (int)done);
-                LAUNCH_CHECK();
-            }
+            const int rc = run_materialised_rows(ctx, (size_t)slow, stride, ctx->gscratch, [&](size_t i0, int n) {
+                k_grid_list<<<(n + 127) / 128, 128, 0, ctx->gstream>>>(ctx->dsys, gp, ctx->gridSlow.as<unsigned long long>() + i0, nullptr,
+                                                                   n, ctx->gscratch.as<double>(), stride, heavy + (int)i0);
+            });
+            if (rc != WVA_OK) return rc;
             listSlots += slow;
         }
         if (leanPending) CK(cudaStreamWaitEvent(ctx->gstream, ctx->evLean, 0));     // join k_scan_lean
@@ -1543,8 +1551,8 @@ static BlockParams block_params(wva_ctx* ctx) {
 }
 
 // Exact chains of list[0, n), then the candidates whose chain met a rescale predicate (and those the scan listed) on
-// the materialised path, in pieces whose p[] scratch fits in half of the free device memory.  The literal list must
-// have room for n more entries than it holds.
+// the materialised path, in chunks under the scratch rule of run_materialised.  The literal list must have room for n
+// more entries than it holds.
 static int block_finish(wva_ctx* ctx, const BlockParams& bp, const unsigned long long* list, size_t n, float* out, int byServer) {
     if (n > 0x7fffffffULL) return fail(ctx, WVA_EINVAL, "blocking: more than 2^31 - 1 exact chains");
     if (n > 0) {
@@ -1557,20 +1565,10 @@ static int block_finish(wva_ctx* ctx, const BlockParams& bp, const unsigned long
     if (lit > bp.lit_cap) return fail(ctx, WVA_ECUDA, "blocking: literal list overflow");
     if (lit == 0) return WVA_OK;
     const long long stride = 11LL * bp.b_max + 1;
-    const size_t per = (size_t)stride * 8;
-    size_t freeB = 0, totB = 0;
-    CK(cudaMemGetInfo(&freeB, &totB));
-    size_t maxItems = std::max<size_t>(ctx->blkScratch.cap / per, (freeB / 2) / per);
-    if (maxItems == 0) return fail(ctx, WVA_ECUDA, "not enough device memory for the materialised chain path");
-    if (maxItems > (size_t)lit) maxItems = (size_t)lit;
-    CK(ctx->blkScratch.ensure(maxItems * per));
-    for (size_t done = 0; done < (size_t)lit; done += maxItems) {
-        const int m = (int)std::min<size_t>((size_t)lit - done, maxItems);
-        k_block_literal<<<(m + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, bp, bp.lit_list + done, m, ctx->blkScratch.as<double>(),
+    return run_materialised_rows(ctx, (size_t)lit, stride, ctx->blkScratch, [&](size_t i0, int m) {
+        k_block_literal<<<(m + 127) / 128, 128, 0, ctx->stream>>>(ctx->dsys, bp, bp.lit_list + i0, m, ctx->blkScratch.as<double>(),
                                                                   stride, out, byServer);
-        LAUNCH_CHECK();
-    }
-    return WVA_OK;
+    });
 }
 
 int wva_grid_blocking_size(const wva_ctx* ctx, size_t* n) {

@@ -84,7 +84,7 @@ k_block_scan(DevSystem sys, BlockParams bp) {
         float* out = bp.plane + base;
         const float qnan = __uint_as_float(WVA_BLOCK_NAN);
         GridServer gs;
-        if (scan_pair_status(sys, s, a, gs) != WVA_CAND_OK) {
+        if (grid_pair_status(sys, s, a, gs) != WVA_CAND_OK) {
             for (int n = 0; n < B; ++n) out[n] = qnan;
         } else {
             ServFormula sf; sf.init(gs.sp, gs.inTok, gs.outTok);
@@ -155,7 +155,7 @@ k_block_exact(DevSystem sys, BlockParams bp, const unsigned long long* __restric
     block_decode(bp, sys.A, id, sl, a, r, b);
     const size_t slot = by_server ? (size_t)sl : (size_t)id;
     GridServer gs;
-    if (scan_pair_status(sys, bp.s0 + sl, a, gs) != WVA_CAND_OK) { out[slot] = __uint_as_float(WVA_BLOCK_NAN); return; }
+    if (grid_pair_status(sys, bp.s0 + sl, a, gs) != WVA_CAND_OK) { out[slot] = __uint_as_float(WVA_BLOCK_NAN); return; }
     ServFormula sf; sf.init(gs.sp, gs.inTok, gs.outTok);
     const float lambda = (gs.totalRate / (float)r) / 1000.0f;
     const double lam = (double)lambda;

@@ -171,14 +171,6 @@ __device__ __forceinline__ ScanBlock scan_block(const DevSystem& sys, const Grid
     k.s = gp.s0 + k.sl;
     return k;
 }
-// pair usable for the sweep?  (status of all its candidates otherwise)
-__device__ __forceinline__ int scan_pair_status(const DevSystem& sys, int s, int a, GridServer& gs) {
-    if (!(pair_lookups_ok(sys, s, a) && is_candidate_accel(sys, s, a))) return WVA_CAND_ERR_PAIR;
-    load_grid_server(sys, s, a, gs);
-    if (gs.inTok < 0 || gs.outTok < 1 || gs.sloTTFT < 0.0f || gs.sloITL < 0.0f || gs.sloTPS < 0.0f) return WVA_CAND_ERR_CONFIG;
-    return WVA_CAND_OK;
-}
-
 __global__ void __launch_bounds__(WVA_SCAN_MAXROWS)
 k_scan_prep(DevSystem sys, GridParams gp) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -190,7 +182,7 @@ k_scan_prep(DevSystem sys, GridParams gp) {
     const int B = gp.b_max, R = gp.r_max;
     if (threadIdx.x == 0) sh_nGood = B;
     GridServer gs;
-    const int blockStatus = scan_pair_status(sys, k.s, k.a, gs);
+    const int blockStatus = grid_pair_status(sys, k.s, k.a, gs);
     const size_t candBase = ((size_t)k.pairLocal * R) * (size_t)B;
     ScanRow* rowInfo = gp.row_info + (size_t)k.pairSlice * R;
     if (blockStatus != WVA_CAND_OK) {
@@ -321,38 +313,6 @@ __device__ __forceinline__ void scan_row_best(ScanBest& best, bool& rowHas, cons
     if (key < best.key) { best.key = key; best.itl = i_; best.ttft = t_; best.rho = r_; }
 }
 
-// block argmin + counters (shared by k_scan_cert / k_scan_lean); slotBase separates the two kernels' slots
-__device__ __forceinline__ void scan_block_reduce(const DevSystem& sys, const GridParams& gp, const GridServer& gs, const ScanBlock& k, const int slot,
-                                                  unsigned long long bestKey, float bestItl, float bestTtft, float bestRho,
-                                                  unsigned long long steps, unsigned long long algSteps, unsigned long long okCount,
-                                                  unsigned long long* sh_key, unsigned long long* sh_cnt) {
-    const int lane = threadIdx.x & 31;
-    unsigned long long warpKey = bestKey;
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long other = __shfl_down_sync(0xffffffffu, warpKey, o);
-        if (other < warpKey) warpKey = other;
-        steps += __shfl_down_sync(0xffffffffu, steps, o);
-        algSteps += __shfl_down_sync(0xffffffffu, algSteps, o);
-        okCount += __shfl_down_sync(0xffffffffu, okCount, o);
-    }
-    if (lane == 0) {
-        if (warpKey != WVA_KEY_NONE) atomicMin(sh_key, warpKey);
-        atomicAdd(&sh_cnt[0], steps); atomicAdd(&sh_cnt[1], algSteps); atomicAdd(&sh_cnt[2], okCount);
-    }
-    __syncthreads();
-    const unsigned long long blockKey = *sh_key;
-    if (blockKey != WVA_KEY_NONE && bestKey == blockKey) {
-        GridSlot sl_; sl_.key = blockKey; sl_.itl = bestItl; sl_.ttft = bestTtft; sl_.rho = bestRho; sl_.sl = k.sl; sl_.pad = 0;
-        const int r = (int)((blockKey >> 14) & 0x3ff) + 1;
-        sl_.cost = gs.accCost * (float)go_muli(gs.numInst, (long long)r);
-        gp.block_slot[slot] = sl_;
-        atomicMin(&gp.keys[k.sl], blockKey);
-    }
-    if (threadIdx.x == 0) {
-        atomicAdd(&gp.counters[0], sh_cnt[0]); atomicAdd(&gp.counters[1], sh_cnt[1]); atomicAdd(&gp.counters[2], sh_cnt[2]);
-    }
-}
-
 // ---- the batch sizes from a row's stop on: frozen exact sums ----------------------------------------------------------
 __global__ void __launch_bounds__(WVA_SCAN_WARPS * 32, 5)
 k_scan_lean(DevSystem sys, GridParams gp) {
@@ -365,7 +325,7 @@ k_scan_lean(DevSystem sys, GridParams gp) {
     __shared__ int sh_next;
     if (threadIdx.x == 0) { sh_key = WVA_KEY_NONE; sh_cnt[0] = sh_cnt[1] = sh_cnt[2] = 0; gp.block_slot[slot].key = WVA_KEY_NONE; sh_next = 0; }
     GridServer gs;
-    if (scan_pair_status(sys, k.s, k.a, gs) != WVA_CAND_OK) return;       // k_scan_prep wrote the pair's status
+    if (grid_pair_status(sys, k.s, k.a, gs) != WVA_CAND_OK) return;       // k_scan_prep wrote the pair's status
     __syncthreads();
     const ScanPairCtx pc = scan_pair_ctx(gs);
     const size_t candBase = ((size_t)k.pairLocal * R) * (size_t)B;
@@ -430,7 +390,7 @@ k_scan_lean(DevSystem sys, GridParams gp) {
         }
         okCount += okRow; algSteps += algRow;
     }
-    scan_block_reduce(sys, gp, gs, k, slot, best.key, best.itl, best.ttft, best.rho, 0ULL, algSteps, okCount, &sh_key, sh_cnt);
+    grid_block_reduce(gp, gs, k.sl, slot, best.key, best.itl, best.ttft, best.rho, 0ULL, algSteps, okCount, &sh_key, sh_cnt);
 }
 
 // ---- the batch sizes before a row's stop: ramp by warp scans + certificate --------------------------------------------
@@ -457,7 +417,7 @@ k_scan_cert(DevSystem sys, GridParams gp) {
     __shared__ int sh_status;
     if (threadIdx.x == 0) {
         GridServer g0;
-        sh_status = scan_pair_status(sys, k.s, k.a, g0);
+        sh_status = grid_pair_status(sys, k.s, k.a, g0);
         if (sh_status == WVA_CAND_OK) { sh_gs = g0; sh_pc = scan_pair_ctx(g0); }
     }
     __syncthreads();
@@ -608,7 +568,7 @@ k_scan_cert(DevSystem sys, GridParams gp) {
             scan_row_best(best, rowHas, rc, feasible, n, itl, ttft, rho);
         }
     }
-    scan_block_reduce(sys, gp, gs, k, slot, best.key, best.itl, best.ttft, best.rho, steps, algSteps, okCount, &sh_key, sh_cnt);
+    grid_block_reduce(gp, gs, k.sl, slot, best.key, best.itl, best.ttft, best.rho, steps, algSteps, okCount, &sh_key, sh_cnt);
 }
 
 }  // namespace wva

@@ -1010,6 +1010,25 @@ struct GridServer {
     bool cert;
 };
 
+__device__ __forceinline__ void zero_metrics(wva_metrics& m) {
+    m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
+    m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
+}
+// QueueAnalyzer.Analyze's metrics from a solved model (queueanalyzer.go:152-173)
+__device__ __forceinline__ void grid_metrics(const SolveStats& so, const GridServer& gs, int b, float rateMax, wva_metrics& m) {
+    const float effConc = effective_concurrency(so.avgServTime, gs.sp, gs.inTok, gs.outTok, b);
+    float rho = so.avgNumInServers / (float)b;
+    rho = go_minf(go_maxf(rho, 0.0f), 1.0f);
+    m.throughput = so.throughput * 1000.0f;
+    m.avg_resp_time = so.avgRespTime;
+    m.avg_wait_time = so.avgWaitTime;
+    m.avg_num_in_serv = so.avgNumInServers;
+    m.avg_prefill_time = prefill_time(gs.sp, gs.inTok, effConc);
+    m.avg_token_time = decode_time(gs.sp, effConc);
+    m.max_rate = rateMax;
+    m.rho = rho;
+}
+
 // QueueAnalyzer.Analyze (queueanalyzer.go:134-174) on a fresh analyzer with MaxBatchSize b,
 // MaxQueueSize 10 b, service rates from the shared-memory table.  A fresh model has p[0] = 0 so
 // the validity test (queuemodel.go:30-31) sees rho = 1: valid iff 1 < K and lambda >= 0.
@@ -1031,17 +1050,7 @@ __device__ __forceinline__ int analyze_table(const ServTable& tb, const GridServ
     if (rc == WVA_SOLVE_DEFER) return -2;                                 // long chain: heavy kernel
     if (rc == WVA_SOLVE_CAREFUL) rc = solve_stream_table(tb, b, K, lambda, tame, st, steps);
     if (rc != WVA_SOLVE_OK) return -1;                                    // literal path
-    float effConc = effective_concurrency(st.avgServTime, gs.sp, gs.inTok, gs.outTok, b);
-    float rho = st.avgNumInServers / (float)b;
-    rho = go_minf(go_maxf(rho, 0.0f), 1.0f);
-    m.throughput = st.throughput * 1000.0f;
-    m.avg_resp_time = st.avgRespTime;
-    m.avg_wait_time = st.avgWaitTime;
-    m.avg_num_in_serv = st.avgNumInServers;
-    m.avg_prefill_time = prefill_time(gs.sp, gs.inTok, effConc);
-    m.avg_token_time = decode_time(gs.sp, effConc);
-    m.max_rate = rateMax;
-    m.rho = rho;
+    grid_metrics(st, gs, b, rateMax, m);
     return WVA_CAND_OK;
 }
 
@@ -1075,6 +1084,57 @@ __device__ __forceinline__ void load_grid_server(const DevSystem& sys, int s, in
     gs.cert = sys.cert != 0;
 }
 
+// pair usable for the sweep?  (status of all its candidates otherwise)
+__device__ __forceinline__ int grid_pair_status(const DevSystem& sys, int s, int a, GridServer& gs) {
+    if (!(pair_lookups_ok(sys, s, a) && is_candidate_accel(sys, s, a))) return WVA_CAND_ERR_PAIR;
+    load_grid_server(sys, s, a, gs);
+    if (gs.inTok < 0 || gs.outTok < 1 || gs.sloTTFT < 0.0f || gs.sloITL < 0.0f || gs.sloTPS < 0.0f) return WVA_CAND_ERR_CONFIG;
+    return WVA_CAND_OK;
+}
+
+// one candidate's cube entry and status byte
+__device__ __forceinline__ void store_candidate(const GridParams& gp, size_t ci, const wva_metrics& m, int status) {
+    if (gp.cube) {
+        float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
+        c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
+        c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
+    }
+    if (gp.status) gp.status[ci] = (unsigned char)status;
+}
+
+// End of every sweep kernel: warp-shuffle then block argmin of the threads' best keys, and the block's counters.  The owner
+// of the block minimum (keys are unique per candidate: one owner) publishes its metrics in gp.block_slot[slot].
+__device__ __forceinline__ void grid_block_reduce(const GridParams& gp, const GridServer& gs, const int sl, const int slot,
+                                                  unsigned long long bestKey, float bestItl, float bestTtft, float bestRho,
+                                                  unsigned long long steps, unsigned long long algSteps, unsigned long long okCount,
+                                                  unsigned long long* sh_key, unsigned long long* sh_cnt) {
+    const int lane = threadIdx.x & 31;
+    unsigned long long warpKey = bestKey;
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long other = __shfl_down_sync(0xffffffffu, warpKey, o);
+        if (other < warpKey) warpKey = other;
+        steps += __shfl_down_sync(0xffffffffu, steps, o);
+        algSteps += __shfl_down_sync(0xffffffffu, algSteps, o);
+        okCount += __shfl_down_sync(0xffffffffu, okCount, o);
+    }
+    if (lane == 0) {
+        if (warpKey != WVA_KEY_NONE) atomicMin(sh_key, warpKey);
+        atomicAdd(&sh_cnt[0], steps); atomicAdd(&sh_cnt[1], algSteps); atomicAdd(&sh_cnt[2], okCount);
+    }
+    __syncthreads();
+    const unsigned long long blockKey = *sh_key;
+    if (blockKey != WVA_KEY_NONE && bestKey == blockKey) {
+        GridSlot sl_; sl_.key = blockKey; sl_.itl = bestItl; sl_.ttft = bestTtft; sl_.rho = bestRho; sl_.sl = sl; sl_.pad = 0;
+        const int r = (int)((blockKey >> 14) & 0x3ff) + 1;
+        sl_.cost = gs.accCost * (float)go_muli(gs.numInst, (long long)r);
+        gp.block_slot[slot] = sl_;
+        atomicMin(&gp.keys[sl], blockKey);
+    }
+    if (threadIdx.x == 0) {
+        atomicAdd(&gp.counters[0], sh_cnt[0]); atomicAdd(&gp.counters[1], sh_cnt[1]); atomicAdd(&gp.counters[2], sh_cnt[2]);
+    }
+}
+
 // Block = one (server, accelerator) pair x one chunk of replica counts.  The pair's service-rate
 // table (float, double and refined reciprocal, 20 B per batch size) is built once into shared
 // memory; warps then pull (replicas, 32 consecutive batch sizes) work items from a shared counter:
@@ -1106,25 +1166,16 @@ k_grid(DevSystem sys, GridParams gp) {
         gp.block_slot[blockIdx.x].key = WVA_KEY_NONE;
     }
 
-    const bool pairOk = pair_lookups_ok(sys, s, a) && is_candidate_accel(sys, s, a);
     GridServer gs;
-    int blockStatus = WVA_CAND_OK;
-    if (!pairOk) blockStatus = WVA_CAND_ERR_PAIR;
-    else {
-        load_grid_server(sys, s, a, gs);
-        if (gs.inTok < 0 || gs.outTok < 1 || gs.sloTTFT < 0.0f || gs.sloITL < 0.0f || gs.sloTPS < 0.0f)
-            blockStatus = WVA_CAND_ERR_CONFIG;
-    }
+    const int blockStatus = grid_pair_status(sys, s, a, gs);
     const size_t candBase = ((size_t)pairLocal * gp.r_max) * (size_t)B;
     if (blockStatus != WVA_CAND_OK) {
         // whole block shares one error status; zero metrics
         if (gp.status || gp.cube) {
             const size_t n = (size_t)(r_hi - r_lo + 1) * B;
             const size_t off = candBase + (size_t)(r_lo - 1) * B;
-            for (size_t i = threadIdx.x; i < n; i += blockDim.x) {
-                if (gp.status) gp.status[off + i] = (unsigned char)blockStatus;
-                if (gp.cube) { float4 z = make_float4(0, 0, 0, 0); float4* c = reinterpret_cast<float4*>(&gp.cube[off + i]); c[0] = z; c[1] = z; }
-            }
+            wva_metrics z; zero_metrics(z);
+            for (size_t i = threadIdx.x; i < n; i += blockDim.x) store_candidate(gp, off + i, z, blockStatus);
         }
         return;
     }
@@ -1167,8 +1218,7 @@ k_grid(DevSystem sys, GridParams gp) {
         const size_t ci = candBase + (size_t)(r - 1) * B + (size_t)(b - 1);
         const float rate = gs.totalRate / (float)r;
         wva_metrics m;
-        m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-        m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
+        zero_metrics(m);
         float rateTPS = 0.0f;
         int st;
         bool feasible = false;
@@ -1199,43 +1249,10 @@ k_grid(DevSystem sys, GridParams gp) {
             if (key < bestKey) {
                 bestKey = key; bestItl = m.avg_token_time; bestTtft = m.avg_wait_time + m.avg_prefill_time; bestRho = m.rho;
             }
-        } else {
-            m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-            m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-        }
-        if (gp.cube) {
-            float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
-            c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
-            c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
-        }
-        if (gp.status) gp.status[ci] = (unsigned char)(st | (feasible ? WVA_CAND_FEASIBLE : 0));
+        } else zero_metrics(m);
+        store_candidate(gp, ci, m, st | (feasible ? WVA_CAND_FEASIBLE : 0));
     }
-
-    // ---- warp-shuffle then block argmin; the owner of the block minimum publishes its metrics ----
-    unsigned long long warpKey = bestKey;
-    for (int o = 16; o > 0; o >>= 1) {
-        unsigned long long other = __shfl_down_sync(0xffffffffu, warpKey, o);
-        if (other < warpKey) warpKey = other;
-        steps += __shfl_down_sync(0xffffffffu, steps, o);
-        algSteps += __shfl_down_sync(0xffffffffu, algSteps, o);
-        okCount += __shfl_down_sync(0xffffffffu, okCount, o);
-    }
-    if (lane == 0) {
-        if (warpKey != WVA_KEY_NONE) atomicMin(&sh_key, warpKey);
-        atomicAdd(&sh_cnt[0], steps); atomicAdd(&sh_cnt[1], algSteps); atomicAdd(&sh_cnt[2], okCount);
-    }
-    __syncthreads();
-    const unsigned long long blockKey = sh_key;
-    if (blockKey != WVA_KEY_NONE && bestKey == blockKey) {          // keys are unique per candidate: one owner
-        GridSlot sl_; sl_.key = blockKey; sl_.itl = bestItl; sl_.ttft = bestTtft; sl_.rho = bestRho; sl_.sl = sl; sl_.pad = 0;
-        const int r = (int)((blockKey >> 14) & 0x3ff) + 1;
-        sl_.cost = gs.accCost * (float)go_muli(gs.numInst, (long long)r);
-        gp.block_slot[blockIdx.x] = sl_;
-        atomicMin(&gp.keys[sl], blockKey);
-    }
-    if (threadIdx.x == 0) {
-        atomicAdd(&gp.counters[0], sh_cnt[0]); atomicAdd(&gp.counters[1], sh_cnt[1]); atomicAdd(&gp.counters[2], sh_cnt[2]);
-    }
+    grid_block_reduce(gp, gs, sl, blockIdx.x, bestKey, bestItl, bestTtft, bestRho, steps, algSteps, okCount, &sh_key, sh_cnt);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1274,31 +1291,21 @@ k_grid_rows(DevSystem sys, GridParams gp) {
     const int B = gp.b_max, R = gp.r_max;
     const int b0 = seg * gp.b_seg;                                   // this block: states b0+1 .. b1
     const int b1 = (b0 + gp.b_seg < B) ? b0 + gp.b_seg : B;
-    const int lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
         sh_nGood = b1; sh_key = WVA_KEY_NONE; sh_cnt[0] = sh_cnt[1] = sh_cnt[2] = 0;
         gp.block_slot[blockIdx.x].key = WVA_KEY_NONE;
     }
-    const bool pairOk = pair_lookups_ok(sys, s, a) && is_candidate_accel(sys, s, a);
     GridServer gs;
-    int blockStatus = WVA_CAND_OK;
-    if (!pairOk) blockStatus = WVA_CAND_ERR_PAIR;
-    else {
-        load_grid_server(sys, s, a, gs);
-        if (gs.inTok < 0 || gs.outTok < 1 || gs.sloTTFT < 0.0f || gs.sloITL < 0.0f || gs.sloTPS < 0.0f)
-            blockStatus = WVA_CAND_ERR_CONFIG;
-    }
+    const int blockStatus = grid_pair_status(sys, s, a, gs);
     const size_t candBase = ((size_t)pairLocal * R) * (size_t)B;
     if (blockStatus != WVA_CAND_OK) {
         if (gp.status || gp.cube) {
             const int w = b1 - b0;
             const size_t n = (size_t)R * w;
-            for (size_t j = threadIdx.x; j < n; j += blockDim.x) {
-                const size_t i = (j / w) * (size_t)B + (size_t)b0 + (j % w);
-                if (gp.status) gp.status[candBase + i] = (unsigned char)blockStatus;
-                if (gp.cube) { float4 z = make_float4(0, 0, 0, 0); float4* c = reinterpret_cast<float4*>(&gp.cube[candBase + i]); c[0] = z; c[1] = z; }
-            }
+            wva_metrics z; zero_metrics(z);
+            for (size_t j = threadIdx.x; j < n; j += blockDim.x)
+                store_candidate(gp, candBase + (j / w) * (size_t)B + (size_t)b0 + (j % w), z, blockStatus);
         }
         return;
     }
@@ -1387,8 +1394,7 @@ k_grid_rows(DevSystem sys, GridParams gp) {
             int st;
             bool feasible = false;
             wva_metrics m;
-            m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-            m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
+            zero_metrics(m);
             if (b > nGood) {                                   // bad table entry: literal path decides
                 int k = atomicAdd(gp.slow_count, 1);
                 if (k < gp.slow_cap) gp.slow_list[k] = (unsigned long long)ci;
@@ -1412,85 +1418,37 @@ k_grid_rows(DevSystem sys, GridParams gp) {
                         certified = cert_eval(c, so);
                     }
                 }
-                if (!certified) {
-                    // exact chain in k_grid_list; when that list is full, right here
+                if (certified) {
+                    st = WVA_CAND_OK;
+                    grid_metrics(so, gs, b, rateMax, m);
+                } else {
+                    // exact chain in k_grid_list; when that list is full, right here (m stays zero unless it is analysed)
                     int k = atomicAdd(gp.heavy_count, 1);
                     if (k < gp.heavy_cap) { gp.heavy_list[k] = (unsigned long long)ci; gp.heavy_cost[k] = (float)K; continue; }
                     ServTable tb; tb.rateF = rateF; tb.rateD = rateD; tb.rcp = rcp;
                     float rt, dc;
-                    int st2 = analyze_table(tb, gs, b, rate, tame, 0, m, rt, steps, dc);
-                    if (st2 < 0) { int k2 = atomicAdd(gp.slow_count, 1); if (k2 < gp.slow_cap) gp.slow_list[k2] = (unsigned long long)ci; continue; }
-                    so.avgServTime = 0.0f;      // metrics already final in m
-                    st = st2;
-                    goto have_metrics;
+                    st = analyze_table(tb, gs, b, rate, tame, 0, m, rt, steps, dc);
+                    if (st < 0) { int k2 = atomicAdd(gp.slow_count, 1); if (k2 < gp.slow_cap) gp.slow_list[k2] = (unsigned long long)ci; continue; }
                 }
-                st = WVA_CAND_OK;
-                {
-                    const float effConc = effective_concurrency(so.avgServTime, gs.sp, gs.inTok, gs.outTok, b);
-                    float rho = so.avgNumInServers / (float)b;
-                    rho = go_minf(go_maxf(rho, 0.0f), 1.0f);
-                    m.throughput = so.throughput * 1000.0f;
-                    m.avg_resp_time = so.avgRespTime;
-                    m.avg_wait_time = so.avgWaitTime;
-                    m.avg_num_in_serv = so.avgNumInServers;
-                    m.avg_prefill_time = prefill_time(gs.sp, gs.inTok, effConc);
-                    m.avg_token_time = decode_time(gs.sp, effConc);
-                    m.max_rate = rateMax;
-                    m.rho = rho;
-                }
-            have_metrics:
-                if (st != WVA_CAND_OK) {
-                    m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-                    m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-                    goto write_out;
-                }
-                okCount++;
-                algSteps += 2ULL * (unsigned long long)(K + 1);
-                const float lamMaxBack = rateMax / 1000.0f;
-                const float rateTPS = (lamMaxBack * (1.0f - WVA_STABILITY_SAFETY)) * 1000.0f;
-                const float ttft = m.avg_wait_time + m.avg_prefill_time;
-                const float itl = m.avg_token_time;
-                feasible = (!(gs.sloTTFT > 0.0f) || ttft <= gs.sloTTFT) && (!(gs.sloITL > 0.0f) || itl <= gs.sloITL) &&
-                           (!(gs.sloTPS > 0.0f) || rate <= rateTPS) && (r >= gs.minReplicas);
-                if (feasible && value == value) {              // a NaN value is never selected
-                    const unsigned long long key = make_key(value, a, r, b);
-                    if (key < bestKey) { bestKey = key; bestItl = itl; bestTtft = ttft; bestRho = m.rho; }
+                if (st == WVA_CAND_OK) {
+                    okCount++;
+                    algSteps += 2ULL * (unsigned long long)(K + 1);
+                    const float lamMaxBack = rateMax / 1000.0f;
+                    const float rateTPS = (lamMaxBack * (1.0f - WVA_STABILITY_SAFETY)) * 1000.0f;
+                    const float ttft = m.avg_wait_time + m.avg_prefill_time;
+                    const float itl = m.avg_token_time;
+                    feasible = (!(gs.sloTTFT > 0.0f) || ttft <= gs.sloTTFT) && (!(gs.sloITL > 0.0f) || itl <= gs.sloITL) &&
+                               (!(gs.sloTPS > 0.0f) || rate <= rateTPS) && (r >= gs.minReplicas);
+                    if (feasible && value == value) {              // a NaN value is never selected
+                        const unsigned long long key = make_key(value, a, r, b);
+                        if (key < bestKey) { bestKey = key; bestItl = itl; bestTtft = ttft; bestRho = m.rho; }
+                    }
                 }
             }
-        write_out:
-            if (gp.cube) {
-                float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
-                c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
-                c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
-            }
-            if (gp.status) gp.status[ci] = (unsigned char)(st | (feasible ? WVA_CAND_FEASIBLE : 0));
+            store_candidate(gp, ci, m, st | (feasible ? WVA_CAND_FEASIBLE : 0));
         }
     }
-    // ---- block argmin + counters ------------------------------------------------------------------
-    unsigned long long warpKey = bestKey;
-    for (int o = 16; o > 0; o >>= 1) {
-        unsigned long long other = __shfl_down_sync(0xffffffffu, warpKey, o);
-        if (other < warpKey) warpKey = other;
-        steps += __shfl_down_sync(0xffffffffu, steps, o);
-        algSteps += __shfl_down_sync(0xffffffffu, algSteps, o);
-        okCount += __shfl_down_sync(0xffffffffu, okCount, o);
-    }
-    if (lane == 0) {
-        if (warpKey != WVA_KEY_NONE) atomicMin(&sh_key, warpKey);
-        atomicAdd(&sh_cnt[0], steps); atomicAdd(&sh_cnt[1], algSteps); atomicAdd(&sh_cnt[2], okCount);
-    }
-    __syncthreads();
-    const unsigned long long blockKey = sh_key;
-    if (blockKey != WVA_KEY_NONE && bestKey == blockKey) {
-        GridSlot sl_; sl_.key = blockKey; sl_.itl = bestItl; sl_.ttft = bestTtft; sl_.rho = bestRho; sl_.sl = sl; sl_.pad = 0;
-        const int r = (int)((blockKey >> 14) & 0x3ff) + 1;
-        sl_.cost = gs.accCost * (float)go_muli(gs.numInst, (long long)r);
-        gp.block_slot[blockIdx.x] = sl_;
-        atomicMin(&gp.keys[sl], blockKey);
-    }
-    if (threadIdx.x == 0) {
-        atomicAdd(&gp.counters[0], sh_cnt[0]); atomicAdd(&gp.counters[1], sh_cnt[1]); atomicAdd(&gp.counters[2], sh_cnt[2]);
-    }
+    grid_block_reduce(gp, gs, sl, blockIdx.x, bestKey, bestItl, bestTtft, bestRho, steps, algSteps, okCount, &sh_key, sh_cnt);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1537,24 +1495,15 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
         sh_hcount = 0; sh_hnext = 0;
         gp.block_slot[blockIdx.x].key = WVA_KEY_NONE;
     }
-    const bool pairOk = pair_lookups_ok(sys, s, a) && is_candidate_accel(sys, s, a);
     GridServer gs;
-    int blockStatus = WVA_CAND_OK;
-    if (!pairOk) blockStatus = WVA_CAND_ERR_PAIR;
-    else {
-        load_grid_server(sys, s, a, gs);
-        if (gs.inTok < 0 || gs.outTok < 1 || gs.sloTTFT < 0.0f || gs.sloITL < 0.0f || gs.sloTPS < 0.0f)
-            blockStatus = WVA_CAND_ERR_CONFIG;
-    }
+    const int blockStatus = grid_pair_status(sys, s, a, gs);
     const size_t candBase = ((size_t)pairLocal * gp.r_max) * (size_t)B;
     if (blockStatus != WVA_CAND_OK) {
         if (gp.status || gp.cube) {
             const size_t n = (size_t)(r_hi - r_lo + 1) * B;
             const size_t off = candBase + (size_t)(r_lo - 1) * B;
-            for (size_t i = threadIdx.x; i < n; i += blockDim.x) {
-                if (gp.status) gp.status[off + i] = (unsigned char)blockStatus;
-                if (gp.cube) { float4 z = make_float4(0, 0, 0, 0); float4* c = reinterpret_cast<float4*>(&gp.cube[off + i]); c[0] = z; c[1] = z; }
-            }
+            wva_metrics z; zero_metrics(z);
+            for (size_t i = threadIdx.x; i < n; i += blockDim.x) store_candidate(gp, off + i, z, blockStatus);
         }
         return;
     }
@@ -1684,8 +1633,7 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
             int st;
             bool feasible = false;
             wva_metrics m;
-            m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-            m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
+            zero_metrics(m);
             if (b > nGood) {                                   // bad table entry: literal path decides
                 int k = atomicAdd(gp.slow_count, 1);
                 if (k < gp.slow_cap) gp.slow_list[k] = (unsigned long long)ci;
@@ -1707,10 +1655,12 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
                         certified = cert_eval(c, so);
                     }
                 }
-                if (!certified) {
-                    // the exact chain: later, by all warps of the block (inline only when the list is full)
+                if (certified) {
+                    st = WVA_CAND_OK;
+                    grid_metrics(so, gs, b, rateMax, m);
+                } else {
                     // the exact chain: in the deferred-chain kernel (one warp per chain, all SMs); only when that
-                    // list is full, in this block's own list below
+                    // list is full, in this block's own list below, and when that is full too, right here
                     {
                         int k = atomicAdd(gp.heavy_count, 1);
                         if (k < gp.heavy_cap) { gp.heavy_list[k] = (unsigned long long)ci; gp.heavy_cost[k] = (float)K; continue; }
@@ -1718,52 +1668,25 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
                     const int hk = atomicAdd(&sh_hcount, 1);
                     if (hk < WVA_WROW_LIST) { sh_heavy[hk] = (r - r_lo) * B + n; continue; }
                     float rt, dc;
-                    int st2 = analyze_table(tb, gs, b, rate, tame, 0, m, rt, steps, dc);
-                    if (st2 < 0) { int k2 = atomicAdd(gp.slow_count, 1); if (k2 < gp.slow_cap) gp.slow_list[k2] = (unsigned long long)ci; continue; }
-                    so.avgServTime = 0.0f;      // metrics already final in m
-                    st = st2;
-                    goto have_metrics;
+                    st = analyze_table(tb, gs, b, rate, tame, 0, m, rt, steps, dc);
+                    if (st < 0) { int k2 = atomicAdd(gp.slow_count, 1); if (k2 < gp.slow_cap) gp.slow_list[k2] = (unsigned long long)ci; continue; }
                 }
-                st = WVA_CAND_OK;
-                {
-                    const float effConc = effective_concurrency(so.avgServTime, gs.sp, gs.inTok, gs.outTok, b);
-                    float rho = so.avgNumInServers / (float)b;
-                    rho = go_minf(go_maxf(rho, 0.0f), 1.0f);
-                    m.throughput = so.throughput * 1000.0f;
-                    m.avg_resp_time = so.avgRespTime;
-                    m.avg_wait_time = so.avgWaitTime;
-                    m.avg_num_in_serv = so.avgNumInServers;
-                    m.avg_prefill_time = prefill_time(gs.sp, gs.inTok, effConc);
-                    m.avg_token_time = decode_time(gs.sp, effConc);
-                    m.max_rate = rateMax;
-                    m.rho = rho;
-                }
-            have_metrics:
-                if (st != WVA_CAND_OK) {
-                    m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-                    m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-                    goto write_out;
-                }
-                okCount++;
-                algSteps += 2ULL * (unsigned long long)(K + 1);
-                const float lamMaxBack = rateMax / 1000.0f;
-                const float rateTPS = (lamMaxBack * (1.0f - WVA_STABILITY_SAFETY)) * 1000.0f;
-                const float ttft = m.avg_wait_time + m.avg_prefill_time;
-                const float itl = m.avg_token_time;
-                feasible = (!(gs.sloTTFT > 0.0f) || ttft <= gs.sloTTFT) && (!(gs.sloITL > 0.0f) || itl <= gs.sloITL) &&
-                           (!(gs.sloTPS > 0.0f) || rate <= rateTPS) && (r >= gs.minReplicas);
-                if (feasible && value == value) {              // a NaN value is never selected
-                    const unsigned long long key = make_key(value, a, r, b);
-                    if (key < bestKey) { bestKey = key; bestItl = itl; bestTtft = ttft; bestRho = m.rho; }
+                if (st == WVA_CAND_OK) {
+                    okCount++;
+                    algSteps += 2ULL * (unsigned long long)(K + 1);
+                    const float lamMaxBack = rateMax / 1000.0f;
+                    const float rateTPS = (lamMaxBack * (1.0f - WVA_STABILITY_SAFETY)) * 1000.0f;
+                    const float ttft = m.avg_wait_time + m.avg_prefill_time;
+                    const float itl = m.avg_token_time;
+                    feasible = (!(gs.sloTTFT > 0.0f) || ttft <= gs.sloTTFT) && (!(gs.sloITL > 0.0f) || itl <= gs.sloITL) &&
+                               (!(gs.sloTPS > 0.0f) || rate <= rateTPS) && (r >= gs.minReplicas);
+                    if (feasible && value == value) {              // a NaN value is never selected
+                        const unsigned long long key = make_key(value, a, r, b);
+                        if (key < bestKey) { bestKey = key; bestItl = itl; bestTtft = ttft; bestRho = m.rho; }
+                    }
                 }
             }
-        write_out:
-            if (gp.cube) {
-                float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
-                c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
-                c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
-            }
-            if (gp.status) gp.status[ci] = (unsigned char)(st | (feasible ? WVA_CAND_FEASIBLE : 0));
+            store_candidate(gp, ci, m, st | (feasible ? WVA_CAND_FEASIBLE : 0));
         }
     }
 
@@ -1784,8 +1707,7 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
             const float rate = gs.totalRate / (float)r;
             const float lambda = rate / 1000.0f;
             wva_metrics m;
-            m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-            m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
+            zero_metrics(m);
             float rateTPS = 0.0f, dc = 0.0f;
             bool feasible = false;
             int st = WVA_CAND_OK;
@@ -1796,17 +1718,7 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
                 const float rateMax = (rateF[n] * (1.0f - WVA_EPSILON)) * 1000.0f;
                 const float lamMaxBack = rateMax / 1000.0f;
                 rateTPS = (lamMaxBack * (1.0f - WVA_STABILITY_SAFETY)) * 1000.0f;
-                const float effConc = effective_concurrency(so.avgServTime, gs.sp, gs.inTok, gs.outTok, b);
-                float rho = so.avgNumInServers / (float)b;
-                rho = go_minf(go_maxf(rho, 0.0f), 1.0f);
-                m.throughput = so.throughput * 1000.0f;
-                m.avg_resp_time = so.avgRespTime;
-                m.avg_wait_time = so.avgWaitTime;
-                m.avg_num_in_serv = so.avgNumInServers;
-                m.avg_prefill_time = prefill_time(gs.sp, gs.inTok, effConc);
-                m.avg_token_time = decode_time(gs.sp, effConc);
-                m.max_rate = rateMax;
-                m.rho = rho;
+                grid_metrics(so, gs, b, rateMax, m);
                 steps += wsteps;
             } else if (lane == 0) {
                 st = analyze_table(tb, gs, b, rate, tame, 0, m, rateTPS, steps, dc);     // per-thread solver, all cases
@@ -1821,44 +1733,11 @@ k_grid_wrow(DevSystem sys, GridParams gp) {
                 if (key < bestKey) {
                     bestKey = key; bestItl = m.avg_token_time; bestTtft = m.avg_wait_time + m.avg_prefill_time; bestRho = m.rho;
                 }
-            } else {
-                m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-                m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-            }
-            if (gp.cube) {
-                float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
-                c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
-                c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
-            }
-            if (gp.status) gp.status[ci] = (unsigned char)(st | (feasible ? WVA_CAND_FEASIBLE : 0));
+            } else zero_metrics(m);
+            store_candidate(gp, ci, m, st | (feasible ? WVA_CAND_FEASIBLE : 0));
         }
     }
-
-    // ---- warp-shuffle then block argmin; the owner of the block minimum publishes its metrics ----
-    unsigned long long warpKey = bestKey;
-    for (int o = 16; o > 0; o >>= 1) {
-        unsigned long long other = __shfl_down_sync(0xffffffffu, warpKey, o);
-        if (other < warpKey) warpKey = other;
-        steps += __shfl_down_sync(0xffffffffu, steps, o);
-        algSteps += __shfl_down_sync(0xffffffffu, algSteps, o);
-        okCount += __shfl_down_sync(0xffffffffu, okCount, o);
-    }
-    if (lane == 0) {
-        if (warpKey != WVA_KEY_NONE) atomicMin(&sh_key, warpKey);
-        atomicAdd(&sh_cnt[0], steps); atomicAdd(&sh_cnt[1], algSteps); atomicAdd(&sh_cnt[2], okCount);
-    }
-    __syncthreads();
-    const unsigned long long blockKey = sh_key;
-    if (blockKey != WVA_KEY_NONE && bestKey == blockKey) {
-        GridSlot sl_; sl_.key = blockKey; sl_.itl = bestItl; sl_.ttft = bestTtft; sl_.rho = bestRho; sl_.sl = sl; sl_.pad = 0;
-        const int r = (int)((blockKey >> 14) & 0x3ff) + 1;
-        sl_.cost = gs.accCost * (float)go_muli(gs.numInst, (long long)r);
-        gp.block_slot[blockIdx.x] = sl_;
-        atomicMin(&gp.keys[sl], blockKey);
-    }
-    if (threadIdx.x == 0) {
-        atomicAdd(&gp.counters[0], sh_cnt[0]); atomicAdd(&gp.counters[1], sh_cnt[1]); atomicAdd(&gp.counters[2], sh_cnt[2]);
-    }
+    grid_block_reduce(gp, gs, sl, blockIdx.x, bestKey, bestItl, bestTtft, bestRho, steps, algSteps, okCount, &sh_key, sh_cnt);
 }
 
 // Candidate evaluated through the formula-based analyzer.  Same arithmetic as analyze_table, hence
@@ -1887,18 +1766,14 @@ __device__ int analyze_candidate(const DevSystem& sys, int s, int a, int r, int 
 //                        the literal list.
 //   scratch != nullptr : the literal list (p[] materialised, `stride` doubles per thread).
 // Each thread publishes key + metrics in gp.list_slot[slot_base + t] for k_grid_claim.
-// one candidate of a list: evaluate, publish key + metrics in gp.list_slot[slot] for k_grid_claim
-__device__ __forceinline__ void grid_list_item(const DevSystem& sys, const GridParams& gp, const size_t ci, const int slotIdx, double* scratchRow,
-                                               unsigned long long& steps, unsigned long long& alg, unsigned long long& okc) {
-    const int B = gp.b_max;
-    const int b = (int)(ci % B) + 1;
-    const int r = (int)((ci / B) % gp.r_max) + 1;
-    const int pairLocal = (int)(ci / ((size_t)B * gp.r_max));
-    const int sl = pairLocal / sys.A, a = pairLocal % sys.A, s = gp.s0 + sl;
-    GridServer gs; wva_metrics m; float rate, rateTPS; int fault = 0;
+
+// Publishes one evaluated candidate of a list: a chain that met a rescale predicate (fault 1) goes to the literal list;
+// otherwise its key (and the server's minimum), the counters and its outputs.  Its slot for k_grid_claim in every case.
+__device__ __forceinline__ void grid_list_publish(const GridParams& gp, const size_t ci, const int slotIdx, const int sl, const int a,
+                                                  const int r, const int b, const int st, const int fault, const GridServer& gs,
+                                                  wva_metrics& m, const float rate, const float rateTPS,
+                                                  unsigned long long& alg, unsigned long long& okc) {
     GridSlot slot; slot.key = WVA_KEY_NONE; slot.cost = slot.itl = slot.ttft = slot.rho = 0.0f; slot.sl = sl; slot.pad = 0;
-    int st = analyze_candidate(sys, s, a, r, b, scratchRow ? nullptr : gp.pair_tab + (size_t)(pairLocal - gp.pair_base) * B,
-                               scratchRow, gs, m, rate, rateTPS, fault, steps);
     if (fault == 1) {
         int k = atomicAdd(gp.slow_count, 1);
         if (k < gp.slow_cap) gp.slow_list[k] = (unsigned long long)ci;
@@ -1913,18 +1788,24 @@ __device__ __forceinline__ void grid_list_item(const DevSystem& sys, const GridP
             }
             alg += 2ULL * (unsigned long long)(11 * b + 1);
             okc += 1;
-        } else {
-            m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-            m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-        }
-        if (gp.cube) {
-            float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
-            c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
-            c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
-        }
-        if (gp.status) gp.status[ci] = (unsigned char)(st | (feasible ? WVA_CAND_FEASIBLE : 0));
+        } else zero_metrics(m);
+        store_candidate(gp, ci, m, st | (feasible ? WVA_CAND_FEASIBLE : 0));
     }
     gp.list_slot[slotIdx] = slot;
+}
+
+// one candidate of a list: evaluate, publish key + metrics in gp.list_slot[slot] for k_grid_claim
+__device__ __forceinline__ void grid_list_item(const DevSystem& sys, const GridParams& gp, const size_t ci, const int slotIdx, double* scratchRow,
+                                               unsigned long long& steps, unsigned long long& alg, unsigned long long& okc) {
+    const int B = gp.b_max;
+    const int b = (int)(ci % B) + 1;
+    const int r = (int)((ci / B) % gp.r_max) + 1;
+    const int pairLocal = (int)(ci / ((size_t)B * gp.r_max));
+    const int sl = pairLocal / sys.A, a = pairLocal % sys.A, s = gp.s0 + sl;
+    GridServer gs; wva_metrics m; float rate, rateTPS; int fault = 0;
+    int st = analyze_candidate(sys, s, a, r, b, scratchRow ? nullptr : gp.pair_tab + (size_t)(pairLocal - gp.pair_base) * B,
+                               scratchRow, gs, m, rate, rateTPS, fault, steps);
+    grid_list_publish(gp, ci, slotIdx, sl, a, r, b, st, fault, gs, m, rate, rateTPS, alg, okc);
 }
 
 __device__ __forceinline__ void grid_list_counters(const GridParams& gp, unsigned long long steps, unsigned long long alg, unsigned long long okc) {
@@ -1993,9 +1874,7 @@ k_grid_list_warp(DevSystem sys, GridParams gp, const unsigned long long* __restr
         for (int i = lane; i < b; i += 32) { const double2 v = tab[i]; rateD[i] = v.x; rcp[i] = v.y; }
         __syncwarp();
         GridServer gs; wva_metrics m; float rate, rateTPS; int fault = 0;
-        m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-        m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-        GridSlot slot; slot.key = WVA_KEY_NONE; slot.cost = slot.itl = slot.ttft = slot.rho = 0.0f; slot.sl = sl; slot.pad = 0;
+        zero_metrics(m);
         load_grid_server(sys, s, a, gs);
         rate = gs.totalRate / (float)r;
         const float lambda = rate / 1000.0f;
@@ -2016,17 +1895,7 @@ k_grid_list_warp(DevSystem sys, GridParams gp, const unsigned long long* __restr
 #endif
             const float lamMaxBack = rateMax / 1000.0f;
             rateTPS = (lamMaxBack * (1.0f - WVA_STABILITY_SAFETY)) * 1000.0f;
-            const float effConc = effective_concurrency(so.avgServTime, gs.sp, gs.inTok, gs.outTok, b);
-            float rho = so.avgNumInServers / (float)b;
-            rho = go_minf(go_maxf(rho, 0.0f), 1.0f);
-            m.throughput = so.throughput * 1000.0f;
-            m.avg_resp_time = so.avgRespTime;
-            m.avg_wait_time = so.avgWaitTime;
-            m.avg_num_in_serv = so.avgNumInServers;
-            m.avg_prefill_time = prefill_time(gs.sp, gs.inTok, effConc);
-            m.avg_token_time = decode_time(gs.sp, effConc);
-            m.max_rate = rateMax;
-            m.rho = rho;
+            grid_metrics(so, gs, b, rateMax, m);
             st = WVA_CAND_OK;
             if (lane == 0) steps += wsteps;
         } else if (lane == 0) {
@@ -2040,32 +1909,7 @@ k_grid_list_warp(DevSystem sys, GridParams gp, const unsigned long long* __restr
         }
         __syncwarp();
         if (lane != 0) continue;
-        if (fault == 1) {
-            int k = atomicAdd(gp.slow_count, 1);
-            if (k < gp.slow_cap) gp.slow_list[k] = (unsigned long long)ci;
-        } else {
-            bool feasible = false;
-            if (st == WVA_CAND_OK) {
-                unsigned long long key = candidate_key(gs, a, r, b, rate, rateTPS, m, feasible);
-                if (key != WVA_KEY_NONE) {
-                    slot.key = key; slot.itl = m.avg_token_time; slot.ttft = m.avg_wait_time + m.avg_prefill_time;
-                    slot.rho = m.rho; slot.cost = gs.accCost * (float)go_muli(gs.numInst, (long long)r);
-                    if (key < gp.keys[sl]) atomicMin(&gp.keys[sl], key);
-                }
-                alg += 2ULL * (unsigned long long)(11 * b + 1);
-                okc += 1;
-            } else {
-                m.throughput = m.avg_resp_time = m.avg_wait_time = m.avg_num_in_serv = 0.0f;
-                m.avg_prefill_time = m.avg_token_time = m.max_rate = m.rho = 0.0f;
-            }
-            if (gp.cube) {
-                float4* c = reinterpret_cast<float4*>(&gp.cube[ci]);
-                c[0] = make_float4(m.throughput, m.avg_resp_time, m.avg_wait_time, m.avg_num_in_serv);
-                c[1] = make_float4(m.avg_prefill_time, m.avg_token_time, m.max_rate, m.rho);
-            }
-            if (gp.status) gp.status[ci] = (unsigned char)(st | (feasible ? WVA_CAND_FEASIBLE : 0));
-        }
-        gp.list_slot[slot_base + t] = slot;
+        grid_list_publish(gp, ci, slot_base + t, sl, a, r, b, st, fault, gs, m, rate, rateTPS, alg, okc);
     }
     if (lane == 0) {
         if (steps) atomicAdd(&gp.counters[0], steps);
@@ -2080,9 +1924,10 @@ __device__ __forceinline__ int heavy_bucket(float cost) {
     k = k < 0 ? 0 : (k > 255 ? 255 : k);
     return 255 - k;
 }
-__global__ void k_heavy_hist(const float* __restrict__ cost, int n, int* __restrict__ hist) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < n) atomicAdd(&hist[heavy_bucket(cost[t])], 1);
+// The list length is read from device memory (*count, clamped to cap), so the launch needs no host round trip.
+__global__ void k_heavy_hist(const float* __restrict__ cost, const int* __restrict__ count, int cap, int* __restrict__ hist) {
+    const int n = min(*count, cap);
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) atomicAdd(&hist[heavy_bucket(cost[t])], 1);
 }
 __global__ void k_heavy_prefix(int* hist /*[256] -> exclusive prefix in place*/) {
     __shared__ int sh[256];
@@ -2093,16 +1938,7 @@ __global__ void k_heavy_prefix(int* hist /*[256] -> exclusive prefix in place*/)
     __syncthreads();
     hist[t] = sh[t];
 }
-__global__ void k_heavy_scatter(const float* __restrict__ cost, int n, int* __restrict__ cursor, int* __restrict__ order) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < n) order[atomicAdd(&cursor[heavy_bucket(cost[t])], 1)] = t;
-}
-// ordering kernels with the list length in device memory
-__global__ void k_heavy_hist_dev(const float* __restrict__ cost, const int* __restrict__ count, int cap, int* __restrict__ hist) {
-    const int n = min(*count, cap);
-    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) atomicAdd(&hist[heavy_bucket(cost[t])], 1);
-}
-__global__ void k_heavy_scatter_dev(const float* __restrict__ cost, const int* __restrict__ count, int cap, int* __restrict__ cursor, int* __restrict__ order) {
+__global__ void k_heavy_scatter(const float* __restrict__ cost, const int* __restrict__ count, int cap, int* __restrict__ cursor, int* __restrict__ order) {
     const int n = min(*count, cap);
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) order[atomicAdd(&cursor[heavy_bucket(cost[t])], 1)] = t;
 }

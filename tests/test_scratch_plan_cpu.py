@@ -1,6 +1,8 @@
 """CPU: the chunk planner of the materialised-p[] path (csrc/wva_scratch_plan.h) compiles without CUDA and lays out
 each chunk's scratch rows as the pair and queue calls need them: prefix sums in list order, one chunk when the list
-fits, a split where the next item would overflow, and an empty chunk when one item alone does not fit."""
+fits, a split where the next item would overflow, and an empty chunk when one item alone does not fit.  Its equal-row
+form, for the sweep's and the blocking plane's lists, covers the list once in order under the same capacity rule:
+the larger of half the free memory and the scratch already held."""
 import os
 import subprocess
 import tempfile
@@ -115,3 +117,82 @@ def test_item_larger_than_capacity_gives_an_empty_chunk(planner):
 def test_empty_list_gives_no_chunks(planner):
     assert planner([], 1 << 30) == []
     assert planner([], 0) == []
+
+
+ROWS_DRIVER = r"""
+#include "wva_scratch_plan.h"
+#include <cstdio>
+// stdin: free bytes, held bytes, n, row doubles.  stdout: one line per chunk, "end doubles", as the runner walks the list
+int main() {
+    size_t freeB = 0, heldB = 0, n = 0;
+    long long row = 0;
+    if (std::scanf("%zu %zu %zu %lld", &freeB, &heldB, &n, &row) != 4) return 2;
+    const long long cap = wva::scratch_cap_doubles(freeB, heldB);
+    for (size_t i0 = 0; i0 < n;) {
+        const wva::ScratchChunk c = wva::scratch_chunk_rows(n, i0, row, cap);
+        std::printf("%zu %lld\n", c.end, c.doubles);
+        if (c.end == i0) break;
+        i0 = c.end;
+    }
+    return 0;
+}
+"""
+
+
+@pytest.fixture(scope="module")
+def rows_planner():
+    """The equal-row planner of the sweep's and the blocking plane's literal lists, under the scratch rule."""
+    with tempfile.TemporaryDirectory() as tmp:
+        src, exe = os.path.join(tmp, "rows.cpp"), os.path.join(tmp, "rows")
+        with open(src, "w") as f:
+            f.write(ROWS_DRIVER)
+        subprocess.check_call([os.environ.get("CXX", "g++"), "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + CSRC,
+                               "-o", exe, src])
+
+        def run(n, row, free, held):
+            out = subprocess.run([exe], input="%d %d %d %d\n" % (free, held, n, row), capture_output=True, text=True,
+                                 check=True).stdout
+            return [tuple(int(x) for x in line.split()) for line in out.splitlines()]
+        yield run
+
+
+def check_rows_cover(chunks, n, row, cap_doubles):
+    start = 0
+    for end, doubles in chunks:
+        assert start < end <= n
+        assert doubles == (end - start) * row <= cap_doubles
+        if end < n:
+            assert doubles + row > cap_doubles
+        start = end
+    assert start == n
+
+
+@pytest.mark.parametrize("n", [1, 7, 1000, 123457])
+def test_equal_rows_cover_the_list_once_in_order(rows_planner, n):
+    row = 11 * 8192 + 1
+    for free in (row * 8 * 2 * 3 + 5, row * 8 * 2 * 1000, 80 << 30):
+        chunks = rows_planner(n, row, free, 0)
+        check_rows_cover(chunks, n, row, (free // 2) // 8)
+        # the parent's rule when nothing is held: (free / 2) / (8 * row) items per chunk
+        assert chunks[0][0] == min(n, (free // 2) // (8 * row))
+
+
+def test_equal_rows_held_scratch_above_half_the_free_memory_gives_the_larger_chunk(rows_planner):
+    row, n = 11 * 512 + 1, 10000
+    free = 2 * 8 * row * 10                    # half the free memory holds 10 rows
+    held = 8 * row * 300                       # the buffer already held holds 300
+    chunks = rows_planner(n, row, free, held)
+    assert chunks[0] == (300, 300 * row)
+    check_rows_cover(chunks, n, row, held // 8)
+    assert len(chunks) == (n + 299) // 300
+    # held memory below half the free memory changes nothing
+    assert rows_planner(n, row, free, 8 * row * 3) == rows_planner(n, row, free, 0)
+    # held memory alone is enough when the free memory is gone
+    assert rows_planner(5, row, 0, 8 * row * 5) == [(5, 5 * row)]
+
+
+def test_equal_row_larger_than_the_capacity_gives_an_empty_chunk(rows_planner):
+    row = 11 * 8192 + 1
+    assert rows_planner(4, row, 2 * 8 * row - 2, 8 * row - 8) == [(0, 0)]
+    assert rows_planner(4, row, 0, 0) == [(0, 0)]
+    assert rows_planner(4, row, 2 * 8 * row, 0) == [(1, row), (2, row), (3, row), (4, row)]
